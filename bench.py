@@ -1,9 +1,10 @@
 #!/usr/bin/env python3
-"""bench.py -- input GB/s scanned by the double-array Aho-Corasick scan path on B200.
+"""bench.py -- input GB/s scanned by the double-array Aho-Corasick scan path on H100.
 
     python bench.py --gpus N --steps K --warmup W                    # headline: C3, find_overlapping_iter
     python bench.py --config {C3,C3-find,C2,C4,C5} ...               # the other BASELINE.json configs
     python bench.py --impl reference [--config ...] ...              # the reference's CPU path (C port)
+    python bench.py ... --dump-outputs DIR                           # also write the last timed step's result
 
 Headline workload (BASELINE.json configs[2] with the headline iterator): a bytewise automaton of 675 000
 UniDic-like patterns; one *step* = one pass of find_overlapping_iter over a batch of 1 Mi haystacks x 4 KiB
@@ -19,6 +20,7 @@ of the crate's loops on the box's host cores, with an in-run parity check of the
 One JSON line is printed by rank 0.  See DESIGN.md section "Measurement" for every field.
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -59,7 +61,7 @@ def measured_peaks():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -79,8 +81,14 @@ class ClockSampler:
                 stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             self.thread = threading.Thread(target=self._read, daemon=True)
             self.thread.start()
+            atexit.register(self._kill)  # a run that fails before stop() must not leave nvidia-smi running
         except Exception:
             self.proc = None
+
+    def _kill(self):
+        if self.proc and self.proc.poll() is None:
+            self.proc.kill()
+            self.proc.wait()
 
     def _read(self):
         for line in self.proc.stdout:
@@ -206,6 +214,40 @@ def mode_ids(mode_name):
             "leftmost_find_iter": (D.LEFTMOST_FIND, O.LEFTMOST_FIND)}[mode_name]
 
 
+DUMP_BYTES = 64 << 20
+DUMP_SEED = 20240901
+
+
+def dump_outputs(out_dir, matches, offsets, hay_len):
+    """Writes what the timed path handed its caller in the last step -- the dense (start, end, value) rows and the
+    n+1 per-haystack offsets -- as float arrays under out_dir, at most DUMP_BYTES in all, so that two builds run with
+    the same arguments can be compared output for output:
+      counts.npy            float32 (n,): matches per haystack (the offsets' differences), every haystack
+      sample_haystacks.npy  float64 (k,): a fixed seeded sample of haystack indices, ascending
+      sample_matches.npy    float64 (m, 3): the rows of those haystacks in output order (cut to fit the budget)
+    matches: (>= total, 3) int32 CUDA tensor, offsets: (n + 1,) int64 CUDA tensor."""
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    o = offsets.cpu().numpy().astype(np.int64)
+    n = len(o) - 1
+    counts = np.diff(o).astype(np.float32)
+    rng = np.random.default_rng(DUMP_SEED)
+    k = min(n, 1024, max(1, (16 << 20) // max(hay_len, 1)))
+    idx = np.sort(rng.choice(n, size=k, replace=False)) if n else np.zeros(0, dtype=np.int64)
+    lens = o[idx + 1] - o[idx]
+    first = np.repeat(o[idx], lens)
+    within = np.arange(int(lens.sum()), dtype=np.int64) - np.repeat(np.cumsum(lens) - lens, lens)
+    budget = (DUMP_BYTES - counts.nbytes - idx.size * 8) // 24
+    rows = (first + within)[:max(budget, 0)]
+    m = np.zeros((0, 3), dtype=np.float64)
+    if rows.size:  # the rows are u32 triples carried in an int32 tensor
+        m = matches[torch.from_numpy(rows).to(matches.device)].cpu().numpy().view(np.uint32).astype(np.float64)
+    np.save(os.path.join(out_dir, "counts.npy"), counts)
+    np.save(os.path.join(out_dir, "sample_haystacks.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "sample_matches.npy"), m.reshape(-1, 3))
+
+
 def cpu_sample(W, opma, omode, n_hay, min_seconds, threads):
     """Times orc_bench_batch on the first n_hay haystacks of the rank's first batch: repeated until min_seconds."""
     import oracle_api as O
@@ -280,9 +322,15 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-overlap", action="store_true", help="one job, placement and next scan serialised (ablation)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's result to DIR/*.npy (see dump_outputs)")
     args = ap.parse_args()
     if args.steps is None:
         args.steps = CONFIGS[args.config]["steps"]
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the GPU path's result (--impl ours)")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -450,6 +498,9 @@ def main():
     job_bytes = step_bytes * world
     value = job_bytes / (ms * 1e-3) / 1e9
     last_batch = (args.warmup + args.steps - 1) % len(batches)
+    if args.dump_outputs and rank == 0:
+        dm, do = group.result(last_total) if group is not None else (out_m, out_o)
+        dump_outputs(args.dump_outputs, dm, do, hay_len)
 
     # ---- in-run parity: the result of the last timed step against the oracle -------------------------------
     # every rank scans a sample of its own shard with the oracle (counts + order-sensitive hashes per haystack,
@@ -558,16 +609,6 @@ def main():
                 "algorithmic_bytes_per_launch": step_bytes, "peak_source": peak_src,
                 "note": "algorithmic bytes = 1 B read per haystack byte x bytes per launch (DESIGN.md); kernel_ms = mean CUDA-event "
                         "time of the scan kernel over the timed steps (events on its launch stream, inside the library)"}
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        try:
-            tj = json.load(open(tpath))
-            ent = tj.get(args.config) or (tj if args.config == "C3" and "dram_bytes_per_byte_scanned" in tj else None)
-            if ent and ent.get("dram_bytes_per_byte_scanned") is not None:
-                roofline["traffic"] = ent["dram_bytes_per_byte_scanned"] * step_bytes
-                roofline["traffic_source"] = ent.get("source", "profiles/traffic.json (ncu --set full capture of this kernel)")
-        except Exception:
-            pass
 
     # ---- CPU baseline: the C port on the host cores, bounded sample -------------------------------------------
     cpu = None
@@ -601,8 +642,8 @@ def main():
                    "image_mib": pma.stats()["image_bytes"] / 2**20, "hay_len": hay_len, "haystacks_per_gpu": n,
                    "bytes_per_gpu": step_bytes, "matches_per_step_per_gpu": counts[last_batch],
                    "matches_per_byte": counts[last_batch] / step_bytes,
-                   "l2": "inputs of consecutive steps (%.2f GiB per GPU before one repeats) are larger than L2 (126 MB); no flush needed" % (
-                       resident / 2**30),
+                   "l2": "inputs of consecutive steps (%.2f GiB per GPU before one repeats) are larger than L2 (%.0f MB); no flush needed" % (
+                       resident / 2**30, torch.cuda.get_device_properties(dev).L2_cache_size / 1e6),
                    "parallelism": "haystack shards, one rank per GPU" + (
                        "; every rank's placement kernel stores its matches into rank 0's dense buffer over NVLink peer memory "
                        "(dach_group_*), rank 0 holds the rebased %d-GPU result after every step" % world if world > 1 else ""),

@@ -1,4 +1,4 @@
-"""daachorse_b200 -- a B200-native (sm_100a) double-array Aho-Corasick scan path that is a
+"""daachorse_b200 -- an H100-native (sm_90a) double-array Aho-Corasick scan path that is a
 drop-in for the scan path of the Rust crate daac-tools/daachorse 4.0.0.
 
 The package holds only what that path needs: ``csrc/`` (CUDA kernels + the C ABI of

@@ -1,4 +1,4 @@
-// CUDA kernels (sm_100a) and the device half of the C ABI of libdaachorse_b200.
+// CUDA kernels (sm_90a) and the device half of the C ABI of libdaachorse_b200.
 //
 // One scan is two phases that only enqueue work (enqueue_scan / enqueue_place; dach_dev_scan_batch runs them back to
 // back on one stream, dach_job_* exposes them, dach_group_* makes the second one the exchange step of a sharded batch):
@@ -185,8 +185,8 @@ __global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
                 for (int k = 0; k < M::TOPUP; ++k) (void)M::step(L, Ev, nullptr);
                 stop = __any_sync(FULL, (L.fl & (F_ACTIVE | M::IDLE)) == (F_ACTIVE | M::IDLE));
             } else if (M::LAZY) {  // look for lanes that need service once per top-up period, not per iteration
-                // (batching further -- wait for four lanes or four periods -- idles ~3 lanes of 32 on
-                // 1 KiB haystacks and lost 6-9 % on the leftmost configs: measured, dropped)
+                // (batching further -- wait for four lanes or four periods -- idles lanes that have
+                // finished short haystacks while the rest of the warp runs on)
                 bool waiting = false;
 #pragma unroll 1
                 for (int k = 0; k < M::TOPUP; ++k) {
@@ -210,8 +210,7 @@ __global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
 
 // ---- StdMachine3, two haystacks per lane ------------------------------------------------------------------
 // The lane machine is latency-bound: one dependent record fetch per lane and iteration, and a warp moves at
-// the pace of its slowest lane (profiles/r2a_*: issue slots 29-47 %, L1 data pipe 36-61 %, LTS 27-52 %,
-// 57-67 % of the stall samples on the fetch's scoreboard).  Here every lane walks TWO independent haystacks:
+// the pace of its slowest lane (most stalls sit on the fetch's scoreboard).  Here every lane walks TWO independent haystacks:
 // both fetches of an iteration are in flight before either result is looked at, so an SM has twice the loads
 // outstanding with the same number of warps.  Lane logic: StdMachine3's probe / resolve, unchanged; the two
 // walkers have their own event queues and take their items from the same counter.
@@ -469,7 +468,7 @@ __global__ void __launch_bounds__(256) k_gather(const uint32_t* pool, const Scan
 // The exchange step proper: `total` dense 12-byte tuples from local memory to out_words + 3 * base in (peer)
 // memory, as DESTINATION-ALIGNED 16-byte stores -- a warp store is 512 contiguous bytes, whole 128-byte lines on
 // NVLink.  (k_gather's own stores are 4 bytes per lane at the 4-byte alignment of a tuple array: as peer stores
-// they reach 350 GB/s into one GPU where the link takes 770, profiles/r2_multi_gpu.md.)
+// they split lines and reach well below what the link takes.)
 // 128 threads x at most 51 registers: two CTAs fit into the registers an SM has left beside a resident scan CTA
 // (1024 threads x 48), so the push of step s really runs while step s+1 is scanned.
 __global__ void __launch_bounds__(128, 10) k_push(const uint32_t* src, const unsigned long long* total_ptr, const unsigned long long* base,
@@ -803,13 +802,14 @@ struct dach_dev {
     // ---- options (dach_dev_set_option) ----
     int64_t opt_slice_mib = 64;
     // Records of the hot region staged in shared memory by StdMachine3 (the region is laid out hottest first, so
-    // any prefix is the best set of its size).  Measured on the C3 bench (profiles/r2_hot_region.md): 9216 staged
-    // records serve 61 % of the fetches and cut the L1 wavefronts per byte by 31 %, yet the kernel gets SLOWER
-    // (124 vs 173 GB/s) -- it is bound by the latency of the fetches that still go to L2, and every KiB of shared
-    // memory is a KiB less L1 for those.  Off by default; -1 = as many as fit next to the event queues.
-    int64_t opt_hot_entries = 0;
+    // any prefix is the best set of its size).  Staged records take fetches off L1 and L2, but every KiB of shared
+    // memory is a KiB less L1 for the fetches that still miss.  On H100 (C3 / C2 A/B, DESIGN.md section 4.1) the
+    // scan kernel gains up to 7168 records (112 KiB beside 80 KiB of queues) and falls off a cliff at 8192, where
+    // the carveout leaves L1 too small for the misses in flight; 6144 keeps a margin.  0 = off, -1 = as many as fit
+    // next to the event queues.
+    int64_t opt_hot_entries = 6144;
     int64_t opt_slice_ramp = 1;      // host path: small slices at the head and the tail of a batch
-    int64_t opt_tail_seg = 0;        // cut only the last 2 x lanes haystacks of a large batch (measured: -2 %, off)
+    int64_t opt_tail_seg = 0;        // cut only the last 2 x lanes haystacks of a large batch (off by default)
     int64_t opt_gather_ordered = 1;  // copy pool blocks in output order (sequential writes)
     int64_t opt_gather_u = 4;     // pooled blocks in flight per warp of k_gather (2, 4 or 8)
     int64_t opt_reserve_sms = 0;  // SMs left free for concurrent kernels
@@ -1427,7 +1427,7 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
     };
     // The copy engine must never wait for the host: the host blocks in scan_locked() until slice k is
     // scanned, so the uploads of the next TWO slices are queued before that (with one slice ahead the
-    // H2D engine idled for the length of every scan: 45 instead of ~55 GB/s).
+    // H2D engine idles for the length of every scan).
     if (!issue_h2d(0)) return DACH_CUDA_ERROR;
     if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
     for (size_t k = 0; k < slices.size(); ++k) {

@@ -1,4 +1,4 @@
-// Per-lane scan logic of libdaachorse_b200 (sm_100a).
+// Per-lane scan logic of libdaachorse_b200 (sm_90a).
 //
 // Everything here is __host__ __device__ so that tests/emu can compile the SAME lane logic
 // with g++ (-DDACH_EMU) and step it on the CPU against the oracle while no GPU is attached.
@@ -139,9 +139,9 @@ struct ScanParams {
 //       these dependent random fetches, and a fetch that misses L2 stalls all 32 lanes of its warp;
 //   [1] haystack text: a lane returns to its 32-byte sector for the next 8 bytes a few microseconds later;
 //   [2] match blocks: written once here, read once by k_gather: evict_first.
-// Without them the text and the match blocks push 6-7 % of the record sectors out of the 126 MB L2
-// (profiles/r1d_*: 2.4 B of DRAM reads per scanned byte, 1.0 of it text).  Option l2_hints: 0 = evict_normal
-// everywhere, 1 = text evict_first, 2 = text evict_normal (profiles/r2_l2_policies.md).
+// Without them the streaming text and match blocks push record sectors out of L2 (50 MB on H100, about
+// the size of a UniDic-scale image).  Option l2_hints: 0 = evict_normal everywhere, 1 = text evict_first,
+// 2 = text evict_normal.
 #if defined(__CUDACC__)
 __constant__ unsigned long long c_l2pol[3];
 #endif
@@ -565,7 +565,7 @@ DACH_HD void scan_leftmost(const ScanParams& P, const RecView& V, TextWin& T, Em
 // The per-byte loop of src/bytewise.rs:1063-1088 is re-cut so that every lane of a warp does the
 // same thing in every iteration: at most ONE 16-byte record fetch, then a short decision.  Lanes
 // walk unrelated haystacks, so a loop shaped like the reference's ("for each byte: while miss:
-// follow fail") leaves ~4 of 32 lanes active per issued instruction (profiles/r1_v0_summary.md);
+// follow fail") leaves only a few of 32 lanes active per issued instruction;
 // here a lane that misses simply spends its next iteration on the next probe of the same byte.
 //
 // Compact record (automata with at most 2^24 slots), 16 bytes:
@@ -651,8 +651,7 @@ DACH_HD uint4 ld_text16(const uint8_t* q, const uint8_t* text_end, const uint8_t
     if (q >= text_end) return w;  // never touch a block that starts past the text
 #if defined(__CUDA_ARCH__)
     // Default: read-only path WITH L1 allocation.  A lane comes back to the same 32-byte sector for
-    // its next 16 bytes; with L1::no_allocate every one of those loads went to DRAM (8.2 GB read per
-    // GiB scanned vs 2.5 GB, profiles/r1_cache_experiments.md).
+    // its next 16 bytes; with L1::no_allocate every one of those loads goes to L2 or DRAM again.
     asm volatile("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
                  : "=r"(w.x), "=r"(w.y), "=r"(w.z), "=r"(w.w)
                  : "l"(q), "l"(c_l2pol[1]));
@@ -1458,7 +1457,7 @@ struct CwMachine {
 
 // =============================================================================================
 // StdMachine2: the bytewise Standard machine again, cut for instruction count (the kernel is
-// issue-bound as much as latency-bound: profiles/r1_final_summary.md, 4.9 warp instructions per byte).
+// issue-bound as much as latency-bound).
 //
 //   * three phases instead of four: a miss computes the address of its next probe on the spot;
 //     fbase of a state whose failure target is ROOT is ROOT's BASE (pre-resolved in the image,
@@ -1688,7 +1687,7 @@ struct StdMachine2 {
 // =============================================================================================
 // StdMachine3: the bytewise Standard machine, third cut -- the default.
 //
-// StdMachine2 sits on two ceilings at once (profiles/r1d_*): the L1 data pipe (every lane's record
+// StdMachine2 sits on two ceilings at once: the L1 data pipe (every lane's record
 // fetch is its own wavefront) and the issue slots (98 warp instructions per lock-step iteration).
 // This cut attacks both:
 //   * records come from the hot-first image (dev_image.cpp): the leading Ev.hot_n slots are staged

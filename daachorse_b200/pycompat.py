@@ -1,5 +1,5 @@
 """The surface of the crate's Python wrapper, daac-tools/python-daachorse (the only other consumer the
-reference names: README.md:19, 223-229), on top of the B200 scan path.
+reference names: README.md:19, 223-229), on top of the GPU scan path.
 
 python-daachorse is a separate repository and is not part of the reference snapshot, so this mirror follows
 its published interface as far as it can be stated from the crate side (SURVEY.md section 8(f) rank 4): one

@@ -1,7 +1,7 @@
 /*
  * daachorse_b200.h -- C ABI of libdaachorse_b200.so
  *
- * A B200-native (sm_100a) double-array Aho-Corasick matcher that is a drop-in for the
+ * An H100-native (sm_90a) double-array Aho-Corasick matcher that is a drop-in for the
  * scan path of the Rust crate daac-tools/daachorse 4.0.0.  The reference has no FFI of
  * its own: its boundary is the crate's public Rust API.  Each entry point below names the
  * reference item it replaces (file:line relative to the crate root) -- INTEGRATION.md
@@ -255,7 +255,7 @@ double dach_dev_last_total_ms(const dach_dev *dev);
 uint64_t dach_dev_last_h2d_bytes(const dach_dev *dev);
 uint64_t dach_dev_last_d2h_bytes(const dach_dev *dev);
 /* Tuning knobs: kernel (3 = StdMachine3, the default; 2, 1 = its predecessors; 0 = lane per haystack),
- * hot_entries (records of the hot region staged in shared memory), threads, ctas_per_sm, seg_len
+ * hot_entries (records of the hot region staged in shared memory, default 6144), threads, ctas_per_sm, seg_len
  * (segment length for intra-haystack chunking of find_overlapping), l2_hints, slice_mib, ... */
 int dach_dev_set_option(dach_dev *dev, const char *name, int64_t value);
 

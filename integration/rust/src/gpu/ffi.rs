@@ -1,5 +1,5 @@
 //! `extern "C"` declarations of libdaachorse_b200 (include/daachorse_b200.h, ABI version 2).
-//! Not compiled in this repository (no Rust toolchain in the build image).
+//! Not compiled in this repository (it builds without a Rust toolchain).
 #![allow(non_camel_case_types)]
 use core::ffi::{c_char, c_void};
 

@@ -1,7 +1,7 @@
-//! `daachorse::gpu`: drop-in twins of the crate's automata whose scans run on a B200.  Same type names, same
+//! `daachorse::gpu`: drop-in twins of the crate's automata whose scans run on an H100.  Same type names, same
 //! constructors (`new`, `with_values`), same iterator methods and `MatchKind` gating; construction stays in the crate,
 //! the serialized automaton crosses the FFI once, haystacks are scanned by libdaachorse_b200.
-//! Not compiled in this repository (no Rust toolchain in the build image).
+//! Not compiled in this repository (it builds without a Rust toolchain).
 //!
 //! Needs two one-line accessors in the crate, `pub(crate) fn match_kind(&self) -> MatchKind { self.match_kind }`
 //! in src/bytewise.rs and src/charwise.rs (the field is private to those modules); `Match`'s fields and

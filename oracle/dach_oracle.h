@@ -7,8 +7,8 @@
  * call it.  Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
  * --impl reference legs use it.
  *
- * Parity pinning: the Rust crate cannot be compiled in this environment (no rustc),
- * so this oracle is pinned against the reference's own fixtures instead (see
+ * Parity pinning: the project builds without a Rust toolchain, so the crate itself is
+ * not run; this oracle is pinned against the reference's own fixtures instead (see
  * tests/test_oracle_golden.py): the 136 SearchTest vectors of
  * tests/aho_corasick_crate_test.rs:63-382 under the 12 configurations at :537-645,
  * the BASE/CHECK/FAIL layout goldens (src/bytewise.rs:1257-1309,
@@ -16,7 +16,7 @@
  * num_states doc constants, the charwise zero-length multibyte vectors, the UTF-8
  * decoder table, the mapper ranks and the serializer LE goldens.
  *
- * All file:line citations are relative to /root/reference/.
+ * All file:line citations are relative to the daachorse 4.0.0 crate root.
  */
 #ifndef DACH_ORACLE_H
 #define DACH_ORACLE_H

@@ -5,7 +5,9 @@ __graft_entry__.smoke() and by bench.py's cpu_baseline / --impl reference legs.
 """
 import ctypes as C
 import os
+import shutil
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -276,16 +278,21 @@ _native = None
 
 
 def native_lib():
-    """liboracle_native.so: the same source built with -march=native ON THIS BOX (the timed CPU baseline);
-    falls back to the portable build if the box has no compiler."""
+    """liboracle_native.so: the same source built with -march=native on the machine that runs it (the timed
+    CPU baseline), in a temporary directory so that the tree may be read-only; falls back to the portable
+    build if the machine has no compiler."""
     global _native
     if _native is None:
-        path = os.path.join(ORACLE_DIR, "liboracle_native.so")
+        tmp = tempfile.mkdtemp(prefix="dach_oracle_")
+        path = os.path.join(tmp, "liboracle_native.so")
         try:
-            subprocess.check_call(["make", "-C", ORACLE_DIR, "-s", "-B", "native"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+            subprocess.check_call(["make", "-C", ORACLE_DIR, "-s", "-B", "native", "NATIVE=" + path],
+                                  stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
             L = C.CDLL(path)
         except Exception:
             L = lib()
+        finally:
+            shutil.rmtree(tmp, ignore_errors=True)  # a loaded library stays mapped
         L.orc_bench_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p,
                                       C.POINTER(C.c_uint64)]
         L.orc_bench_batch.restype = C.c_int

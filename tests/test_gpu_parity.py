@@ -430,11 +430,13 @@ def test_segmented_scan_equals_sequential():
 def test_tail_segmentation_many_small_haystacks():
     """More than 4 haystacks per lane: only the last 2 x lanes haystacks are cut into segments
     (dev_scan.cu, scan_locked); ragged lengths, the longest haystacks sit in the tail."""
+    import torch
+
     cfg = S.config("C2")
     ps = S.make_patterns(cfg, n=3000)
     pool, b = S.make_pool(cfg, ps, 8 << 20)
     rng = np.random.default_rng(11)
-    n = 4 * 148 * 1024 + 5000
+    n = 4 * torch.cuda.get_device_properties(0).multi_processor_count * 1024 + 5000  # lanes = SMs x 1024 threads
     lens = rng.integers(0, 96, size=n)
     lens[-3000:] = rng.integers(2000, 9000, size=3000)
     lens[-1] = 0

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""A/B timing of kernel options on ONE box (boxes of the pool differ by a few percent, so variants are only
-comparable inside one call): builds the C3 batch once, then times the device-resident find_overlapping step
+"""A/B timing of kernel options on ONE GPU (machines differ by a few percent, so variants are only comparable
+inside one run): builds the C3 batch once, then times the device-resident find_overlapping step
 for every option set given on the command line.
 
     python tools/ab_bench.py [--scale 0.25] [--config C3] [--reps 5] "kernel=3" "kernel=3,hot_entries=0" "kernel=2"
@@ -42,7 +42,7 @@ out = torch.empty((r.matches.shape[0] + 1024, 3), dtype=torch.int32, device="cud
 oo = torch.empty(offs_t.numel(), dtype=torch.int64, device="cuda")
 base_sum = int(r.matches.to(torch.int64).sum().item())
 nb = text_t.numel()
-DEFAULTS = {"kernel": 3, "hot_entries": 0, "threads": 1024, "ctas_per_sm": 1, "l2_hints": 2, "gather_ordered": 1}
+DEFAULTS = {"kernel": 3, "hot_entries": 6144, "threads": 1024, "ctas_per_sm": 1, "l2_hints": 2, "gather_ordered": 1}
 for s in (a.sets or ["kernel=3"]):
     opts = dict(DEFAULTS)
     for kv in s.split(","):
