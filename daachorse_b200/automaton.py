@@ -353,6 +353,102 @@ class _Automaton:
             _check(rc)
             return BatchResult(out[: need.value], out_offs)
 
+    # -- counts and first matches (no match list) -------------------------------------------------
+    def _host_batch_args(self, mode, text, offs):
+        self._assert_mode(mode)
+        text = np.ascontiguousarray(text, dtype=np.uint8)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        n = len(offs) - 1
+        if n < 0 or (n > 0 and int(offs.max()) > text.size):
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "offsets must hold n + 1 entries and stay inside the text")
+        return text, offs, n
+
+    def count_batch_host(self, mode, text, offs, device=None):
+        """Matches per haystack of iterator ``mode``, host buffers in and out: ``(np.uint64[n], total)``.
+        counts[i] equals the length of haystack i's run in ``scan_batch_host``; nothing is stored per match."""
+        text, offs, n = self._host_batch_args(mode, text, offs)
+        L = _lib.load()
+        d = self.device_handle(device)
+        counts = np.zeros(n, dtype=np.uint64)
+        total = C.c_uint64()
+        _check(L.dach_count_batch_host(d, mode, _ptr(text), C.c_void_p(offs.ctypes.data), n, _ptr(counts), C.byref(total)))
+        return counts, int(total.value)
+
+    def first_batch_host(self, mode, text, offs, device=None):
+        """First match of iterator ``mode`` on every haystack: ``(MATCH_DTYPE[n], bool[n])``.  Where there is
+        none, found is False and the tuple is all-ones.  The scan of a haystack stops at its first match."""
+        text, offs, n = self._host_batch_args(mode, text, offs)
+        L = _lib.load()
+        d = self.device_handle(device)
+        first = np.zeros(n, dtype=MATCH_DTYPE)
+        found = np.zeros(n, dtype=np.uint8)
+        nf = C.c_uint64()
+        _check(L.dach_first_batch_host(d, mode, _ptr(text), C.c_void_p(offs.ctypes.data), n, _ptr(first), _ptr(found), C.byref(nf)))
+        return first, found.astype(bool)
+
+    def count_batch_device(self, mode, text, offs, out=None, stream=None):
+        """Device-resident form of ``count_batch_host``: ``text`` / ``offs`` as in ``scan_batch_device``;
+        returns an int64 CUDA tensor of n counts (``out``: optional preallocated one)."""
+        import torch
+
+        self._assert_mode(mode)
+        dev = text.device.index if text.device.index is not None else torch.cuda.current_device()
+        n = offs.numel() - 1
+        if out is None and n >= 0:
+            out = torch.empty(n, dtype=torch.int64, device=text.device)
+        _check_device_batch(text, offs, dev, counts=out)
+        d = self.device_handle(dev)
+        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
+        total = C.c_uint64()
+        _check(_lib.load().dach_dev_count_batch(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
+                                                C.c_void_p(out.data_ptr()), C.byref(total), st))
+        return out
+
+    def first_batch_device(self, mode, text, offs, out=None, found=None, stream=None):
+        """Device-resident form of ``first_batch_host``: returns ``(first, found)`` CUDA tensors -- (n, 3) int32
+        carrying the u32 tuples and a bool (n) (``out`` / ``found``: optional preallocated ones)."""
+        import torch
+
+        self._assert_mode(mode)
+        dev = text.device.index if text.device.index is not None else torch.cuda.current_device()
+        n = offs.numel() - 1
+        if out is None and n >= 0:
+            out = torch.empty((n, 3), dtype=torch.int32, device=text.device)
+        if found is None and n >= 0:
+            found = torch.empty(n, dtype=torch.bool, device=text.device)
+        _check_device_batch(text, offs, dev, first=out, found=found)
+        d = self.device_handle(dev)
+        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
+        nf = C.c_uint64()
+        _check(_lib.load().dach_dev_first_batch(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
+                                                C.c_void_p(out.data_ptr()), C.c_void_p(found.data_ptr()), C.byref(nf), st))
+        return out, found
+
+    def _default_mode(self, mode):
+        if mode is not None:
+            return mode
+        return FIND_OVERLAPPING if self.match_kind() == MatchKind.Standard else LEFTMOST_FIND
+
+    def count_batch(self, haystacks, mode=None):
+        """Matches per haystack (np.uint64[n]); ``mode=None``: find_overlapping for Standard automata,
+        leftmost_find for leftmost ones."""
+        blob, offs = _pack(list(haystacks), self._charwise)
+        return self.count_batch_host(self._default_mode(mode), blob, offs)[0]
+
+    def first_match_batch(self, haystacks):
+        """``[Match | None]``: what ``find_iter(h).next()`` (Standard) or ``leftmost_find_iter(h).next()`` gives."""
+        blob, offs = _pack(list(haystacks), self._charwise)
+        first, found = self.first_batch_host(self._default_mode(None), blob, offs)
+        return [Match(m["start"], m["end"], m["value"]) if f else None for m, f in zip(first, found)]
+
+    def is_match_batch(self, haystacks):
+        """np.bool_[n]: does haystack i contain any pattern (the empty pattern included)."""
+        blob, offs = _pack(list(haystacks), self._charwise)
+        return self.first_batch_host(self._default_mode(None), blob, offs)[1]
+
+    def is_match(self, haystack):
+        return bool(self.is_match_batch([haystack])[0])
+
     def job(self, device=None):
         """An asynchronous scan with its own workspace (dach_job_*): ``scan`` and ``place`` only enqueue work,
         ``wait`` blocks.  Several jobs of one automaton overlap across streams and host threads."""
@@ -463,7 +559,8 @@ def torch_int64():
     return torch.int64
 
 
-def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=None, pos=None):
+def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=None, pos=None, counts=None, first=None,
+                        found=None):
     """Raw pointers cross the C ABI: a wrong dtype, stride or device would be silent garbage or a device fault."""
     import torch
 
@@ -475,7 +572,9 @@ def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=No
         bad("offs must hold n + 1 entries")
     for name, t, dtypes in (("text", text, (torch.uint8,)), ("offs", offs, (torch.int64, torch.uint64)),
                             ("out", out, (torch.int32, torch.uint32)), ("out_offs", out_offs, (torch.int64, torch.uint64)),
-                            ("state", state, (torch.int32, torch.uint32)), ("pos", pos, (torch.int32, torch.uint32))):
+                            ("state", state, (torch.int32, torch.uint32)), ("pos", pos, (torch.int32, torch.uint32)),
+                            ("counts", counts, (torch.int64, torch.uint64)), ("first", first, (torch.int32, torch.uint32)),
+                            ("found", found, (torch.bool, torch.uint8))):
         if t is None:
             continue
         if not t.is_cuda or t.device.index != dev_index:
@@ -488,9 +587,11 @@ def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=No
         bad("out must have shape (capacity, 3)")
     if out_offs is not None and out_offs.numel() < n + 1:
         bad("out_offs must hold n + 1 entries")
-    for name, t in (("state", state), ("pos", pos)):
+    for name, t in (("state", state), ("pos", pos), ("counts", counts), ("found", found)):
         if t is not None and t.numel() != n:
             bad("%s must hold n entries" % name)
+    if first is not None and (first.dim() != 2 or first.shape[0] != n or first.shape[1] != 3):
+        bad("first must have shape (n, 3)")
 
 
 def _current_device():

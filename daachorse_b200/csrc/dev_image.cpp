@@ -383,7 +383,11 @@ int build_image(const dach_pma* p, HostImage* img) {
         img->outputs[i * 4 + 0] = p->outputs[i].value;
         img->outputs[i * 4 + 1] = p->outputs[i].length;
         img->outputs[i * 4 + 2] = p->outputs[i].parent;
-        img->outputs[i * 4 + 3] = 0;
+        // the length of the list that starts here (this record and its parents): what a count of
+        // find_overlapping adds per event without walking the list.  A parent comes before its child
+        // (deserialize checks parent < own 1-based index), so it is known already.
+        const uint32_t par = p->outputs[i].parent;
+        img->outputs[i * 4 + 3] = 1u + (par ? img->outputs[(size_t)(par - 1) * 4 + 3] : 0u);
     }
     return DACH_OK;
 }

@@ -12,6 +12,8 @@
 //       k_scan_duo<MODE>        StdMachine3 with two haystacks per lane (option kernel = 4; measured slower)
 //       k_scan<CHARWISE, MODE>  lane per haystack, reference-shaped loop: automata above 2^24 slots, find_iter with
 //                               an empty pattern, and option kernel = 0
+//     k_scan_machine_rk / k_scan_rk  the same machines / loops with a COUNT or FIRST sink (dach_dev_count_batch,
+//                               dach_dev_first_batch), followed by k_count_hay / k_first_hay (per-haystack results)
 //     k_offsets_*               exclusive scan of the per-item match counts
 //     k_blk_index               pool blocks listed in output order (large batches)
 //   phase 2
@@ -54,8 +56,12 @@ constexpr int kMaxThreads = 1024;
 constexpr int kMaxDevices = 64;
 constexpr uint32_t kRootBytes = 1024;  // 256 x u32 at the front of dynamic shared memory
 
-template <bool CHARWISE, int MODE>
-__global__ void __launch_bounds__(kMaxThreads, 1) k_scan(ScanParams P) {
+// the result sink of each result kind
+template <int RK>
+using SinkOf = typename std::conditional<RK == RK_COUNT, CountSink, typename std::conditional<RK == RK_FIRST, FirstSink, Emitter>::type>::type;
+
+template <bool CHARWISE, int MODE, class SINK>
+__device__ __forceinline__ void scan_items(const ScanParams& P) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     uint32_t* s_root = reinterpret_cast<uint32_t*>(smem_raw);
     uint4* s_hot = reinterpret_cast<uint4*>(smem_raw + kRootBytes);
@@ -65,7 +71,7 @@ __global__ void __launch_bounds__(kMaxThreads, 1) k_scan(ScanParams P) {
 
     RecView V{P.rec, s_hot, P.hot_n, s_root};
     TextWin T;
-    Emitter E;
+    SINK E;
     for (;;) {
         const unsigned long long item = bump_u64(&P.ctrl->next_item);
         if (item >= P.n_items) break;
@@ -79,6 +85,16 @@ __global__ void __launch_bounds__(kMaxThreads, 1) k_scan(ScanParams P) {
             scan_standard<CHARWISE, MODE>(P, V, T, E, len);
         E.finish(P);
     }
+}
+
+template <bool CHARWISE, int MODE>
+__global__ void __launch_bounds__(kMaxThreads, 1) k_scan(ScanParams P) {
+    scan_items<CHARWISE, MODE, Emitter>(P);
+}
+// COUNT / FIRST (result kind RK) on the lane-per-haystack loops
+template <bool CHARWISE, int MODE, int RK>
+__global__ void __launch_bounds__(kMaxThreads, 1) k_scan_rk(ScanParams P) {
+    scan_items<CHARWISE, MODE, SinkOf<RK>>(P);
 }
 
 // ---- v1: warp-synchronous lane machine for the bytewise Standard modes ---------------------------
@@ -117,10 +133,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // M: the lane machine (StdMachine3 / StdMachine2 / StdMachine / LmMachine / CwMachine), LANE: its per-lane state.
+// OPS: where drain() and begin_item() come from (M itself for matches, SinkOps for COUNT / FIRST), SINK: the result.
 // HOT: the leading P.hot_entries compact records (the front of the hot region, dev_image.cpp) are staged in
 // shared memory by TMA bulk copies and served from there (StdMachine3).
-template <class M, class LANE, int MAXT, int MINB, bool HOT>
-__global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
+template <class M, class OPS, class LANE, class SINK, bool HOT>
+__device__ __forceinline__ void scan_machine(const ScanParams& P) {
     // dynamic shared memory: [hot records hot_entries x 16 B (HOT only)][event queues LANE_Q x blockDim x 8 B]
     extern __shared__ __align__(128) unsigned char smem_raw[];
     uint4* s_hot = reinterpret_cast<uint4*>(smem_raw);
@@ -147,14 +164,14 @@ __global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
     LANE L;
     L.fl = M::IDLE;
     L.qn = 0;
-    Emitter E;
+    SINK E;
     E.begin(0);
     bool exhausted = false;
     const unsigned long long n_items = P.n_items_dev ? *P.n_items_dev : P.n_items;
     if (HOT) mbar_wait(&s_bar, 0);
     for (;;) {
         // ---- service phase (the warp is converged here) ----
-        if (L.fl & F_ACTIVE) M::drain(L, Ev, P, E);
+        if (L.fl & F_ACTIVE) OPS::drain(L, Ev, P, E);
         if ((L.fl & (F_ACTIVE | F_DONE)) == (F_ACTIVE | F_DONE)) {
             E.finish(P);
             M::finish_item(L, P);
@@ -170,7 +187,7 @@ __global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
             if (need) {
                 const unsigned long long item = base + __popc(m & ((1u << lane) - 1u));
                 if (item < n_items)
-                    M::begin_item(L, P, Ev, E, item, nullptr);
+                    OPS::begin_item(L, P, Ev, E, item, nullptr);
                 else
                     exhausted = true;
             }
@@ -206,6 +223,16 @@ __global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
             }
         }
     }
+}
+
+template <class M, class LANE, int MAXT, int MINB, bool HOT>
+__global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
+    scan_machine<M, M, LANE, Emitter, HOT>(P);
+}
+// COUNT / FIRST (result kind RK) on the lane machine M running iterator MODE
+template <class M, class LANE, int MODE, int RK, bool HOT>
+__global__ void __launch_bounds__(1024, 1) k_scan_machine_rk(ScanParams P) {
+    scan_machine<M, SinkOps<M, MODE, RK>, LANE, SinkOf<RK>, HOT>(P);
 }
 
 // ---- StdMachine3, two haystacks per lane ------------------------------------------------------------------
@@ -665,6 +692,44 @@ __global__ void __launch_bounds__(256) k_seg_fill(const unsigned long long* seg_
     }
 }
 
+// ---- COUNT / FIRST: per-haystack results from per-item results -----------------------------------------------
+// The items of haystack h are [seg_first[h], seg_first[h + 1]) (nullptr: item h alone).  A haystack's count is the
+// sum over its segments, its first match the one of its lowest segment that has one; the totals go to *total.
+__device__ __forceinline__ void add_block_total(unsigned long long v, unsigned long long* total) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_down_sync(0xffffffffu, v, d);
+    if ((threadIdx.x & 31) == 0 && v) atomicAdd(total, v);
+}
+
+__global__ void __launch_bounds__(256) k_count_hay(const unsigned long long* seg_first, const unsigned long long* item_count, uint64_t n,
+                                                    unsigned long long* counts, unsigned long long* total) {
+    const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long v = 0;
+    if (h < n) {
+        const uint64_t lo = seg_first ? seg_first[h] : h, hi = seg_first ? seg_first[h + 1] : h + 1;
+        for (uint64_t i = lo; i < hi; ++i) v += item_count[i];
+        counts[h] = v;
+    }
+    add_block_total(v, total);
+}
+
+__global__ void __launch_bounds__(256) k_first_hay(const unsigned long long* seg_first, const uint4* item_first, uint64_t n,
+                                                    uint32_t* first_words, uint8_t* found, unsigned long long* n_found) {
+    const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long v = 0;
+    if (h < n) {
+        const uint64_t lo = seg_first ? seg_first[h] : h, hi = seg_first ? seg_first[h + 1] : h + 1;
+        uint4 r = item_first[lo];
+        for (uint64_t i = lo + 1; i < hi && !r.w; ++i) r = item_first[i];
+        first_words[h * 3 + 0] = r.x;  // all-ones when there is no match (the sinks start that way)
+        first_words[h * 3 + 1] = r.y;
+        first_words[h * 3 + 2] = r.z;
+        found[h] = r.w ? 1 : 0;
+        v = r.w ? 1 : 0;
+    }
+    add_block_total(v, n_found);
+}
+
 }  // namespace dach
 
 // ------------------------------------------------------------------------------------------
@@ -700,7 +765,8 @@ bool ensure(DevBuf& b, size_t bytes) {
 struct HostPinned {
     unsigned long long total;
     ScanCtrl ctrl;
-    unsigned long long tail_offs[2];  // offs[seg_from], offs[n]: exact size of the segmented tail
+    unsigned long long tail_offs[2];
+    unsigned long long total_rk;  // COUNT / FIRST: total count / haystacks with a match  // offs[seg_from], offs[n]: exact size of the segmented tail
 };
 
 // Everything one in-flight scan needs besides the automaton image.  A scan runs in two phases that may sit on
@@ -711,6 +777,7 @@ struct Workspace {
     DevBuf nseg, seg_first, item_hay, item_beg, item_offs, n_items_dev;  // segment table, per-item offsets
     DevBuf blk_first, blkmap, tiles2;  // pool blocks in output order (k_blk_index)
     DevBuf stage;  // shard groups: the job's dense matches, pushed to the gathering rank by k_push
+    DevBuf items_rk, total_rk;  // COUNT / FIRST: per-item results, the batch's total (u64)
     HostPinned* pinned = nullptr;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // pipeline start, scan end, pipeline end, scan start
     cudaEvent_t ev_scanned = nullptr, ev_placed = nullptr;
@@ -741,7 +808,7 @@ struct Workspace {
     }
     void release() {
         for (DevBuf* b : {&counts, &tiles, &ctrl, &pool, &text, &offs, &out, &out_offs, &nseg, &seg_first, &item_hay, &item_beg,
-                          &item_offs, &n_items_dev, &blk_first, &blkmap, &tiles2, &stage})
+                          &item_offs, &n_items_dev, &blk_first, &blkmap, &tiles2, &stage, &items_rk, &total_rk})
             if (b->p) {
                 cudaFree(b->p);
                 b->p = nullptr;
@@ -963,6 +1030,83 @@ cudaError_t launch_scan(bool cw, int mode, const ScanParams& P, int grid, int th
     return cudaErrorInvalidValue;
 }
 
+// ---- COUNT / FIRST launchers: StdMachine3, LmMachine, CwMachine, or the lane-per-haystack kernels --------------
+template <class M, class LANE, int MODE, int RK, bool HOT>
+cudaError_t launch_rk_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
+    static bool attr_done[kMaxDevices] = {};  // per instantiation and per device
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
+        cudaError_t e = cudaFuncSetAttribute(k_scan_machine_rk<M, LANE, MODE, RK, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+        if (e != cudaSuccess) return e;
+        if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
+    }
+    k_scan_machine_rk<M, LANE, MODE, RK, HOT><<<grid, threads, smem, st>>>(P);
+    return cudaGetLastError();
+}
+template <bool CW, int MODE, int RK>
+cudaError_t launch_scan_rk_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
+    static bool attr_done[kMaxDevices] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
+        cudaError_t e = cudaFuncSetAttribute(k_scan_rk<CW, MODE, RK>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+        if (e != cudaSuccess) return e;
+        if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
+    }
+    k_scan_rk<CW, MODE, RK><<<grid, threads, smem, st>>>(P);
+    return cudaGetLastError();
+}
+
+// which: 3 StdMachine3 (bytewise Standard), 1 LmMachine / CwMachine (by the automaton), 0 lane per haystack.
+// FIRST only runs M_OVERLAPPING (Standard) and M_LEFTMOST: the caller folds the Standard modes.
+template <int RK>
+cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
+    if (which == 3) {
+        switch (mode) {
+            case M_FIND:
+                if constexpr (RK == RK_COUNT)
+                    return P.hot_entries ? launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, RK, true>(P, grid, threads, smem, st)
+                                         : launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, RK, false>(P, grid, threads, smem, st);
+                break;
+            case M_NO_SUFFIX:
+                if constexpr (RK == RK_COUNT)
+                    return P.hot_entries ? launch_rk_t<StdMachine3<M_NO_SUFFIX>, Lane3, M_NO_SUFFIX, RK, true>(P, grid, threads, smem, st)
+                                         : launch_rk_t<StdMachine3<M_NO_SUFFIX>, Lane3, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
+                break;
+            case M_OVERLAPPING:
+                return P.hot_entries ? launch_rk_t<StdMachine3<M_OVERLAPPING>, Lane3, M_OVERLAPPING, RK, true>(P, grid, threads, smem, st)
+                                     : launch_rk_t<StdMachine3<M_OVERLAPPING>, Lane3, M_OVERLAPPING, RK, false>(P, grid, threads, smem, st);
+        }
+        return cudaErrorInvalidValue;
+    }
+    if (which == 1 && cw) {
+        switch (mode) {
+            case M_FIND:
+                if constexpr (RK == RK_COUNT) return launch_rk_t<CwMachine<M_FIND>, LaneCw, M_FIND, RK, false>(P, grid, threads, smem, st);
+                break;
+            case M_NO_SUFFIX:
+                if constexpr (RK == RK_COUNT) return launch_rk_t<CwMachine<M_NO_SUFFIX>, LaneCw, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
+                break;
+            case M_OVERLAPPING: return launch_rk_t<CwMachine<M_OVERLAPPING>, LaneCw, M_OVERLAPPING, RK, false>(P, grid, threads, smem, st);
+            case M_LEFTMOST: return launch_rk_t<CwMachine<M_LEFTMOST>, LaneCw, M_LEFTMOST, RK, false>(P, grid, threads, smem, st);
+        }
+        return cudaErrorInvalidValue;
+    }
+    if (which == 1) return mode == M_LEFTMOST ? launch_rk_t<LmMachine, LaneLm, M_LEFTMOST, RK, false>(P, grid, threads, smem, st) : cudaErrorInvalidValue;
+    switch ((cw ? 4 : 0) + mode) {
+        case 0: if constexpr (RK == RK_COUNT) return launch_scan_rk_t<false, M_FIND, RK>(P, grid, threads, smem, st); break;
+        case 1: return launch_scan_rk_t<false, M_OVERLAPPING, RK>(P, grid, threads, smem, st);
+        case 2: if constexpr (RK == RK_COUNT) return launch_scan_rk_t<false, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
+        case 3: return launch_scan_rk_t<false, M_LEFTMOST, RK>(P, grid, threads, smem, st);
+        case 4: if constexpr (RK == RK_COUNT) return launch_scan_rk_t<true, M_FIND, RK>(P, grid, threads, smem, st); break;
+        case 5: return launch_scan_rk_t<true, M_OVERLAPPING, RK>(P, grid, threads, smem, st);
+        case 6: if constexpr (RK == RK_COUNT) return launch_scan_rk_t<true, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
+        case 7: return launch_scan_rk_t<true, M_LEFTMOST, RK>(P, grid, threads, smem, st);
+    }
+    return cudaErrorInvalidValue;
+}
+
 int check_mode(const dach_dev* d, int mode) {
     if (mode < DACH_FIND || mode > DACH_LEFTMOST_FIND) {
         set_error("unknown scan mode");
@@ -985,6 +1129,82 @@ bool install_policies(int hints) {
     bool ok = cuda_ok(cudaMemcpy(h_pol, d_pol, 24, cudaMemcpyDeviceToHost), "read policies");
     cudaFree(d_pol);
     return ok && cuda_ok(cudaMemcpyToSymbol(c_l2pol, h_pol, 24), "install policies");
+}
+
+// the automaton image and the batch of a scan's ScanParams (results, options and the segment table are set by the caller)
+ScanParams image_params(const dach_dev* d, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
+                        const uint64_t* d_offs, uint64_t n) {
+    ScanParams P;
+    memset(&P, 0, sizeof(P));
+    P.rec = d->d_rec;
+    P.outputs = d->d_outputs;
+    P.root_table = d->d_root;
+    P.crec = d->d_crec;
+    P.opos_tab = d->d_opos;
+    P.root_base = d->root_base;
+    P.mapper = d->d_mapper;
+    P.mapper_len = d->mapper_len;
+    P.n_slots = d->n_slots;
+    P.id_in = d->d_id_in;
+    P.id_out = d->d_id_out;
+    P.root_opos = d->root_opos;
+    P.text = d_text;
+    P.text_lo = text_lo;
+    P.text_end = text_end;
+    P.offs = d_offs;
+    P.n_items = n;
+    return P;
+}
+
+// dynamic shared memory of the scan kernel: the lane machines' event queues (queue_sets per lane) and, for
+// StdMachine3, the front of the hot region; the lane-per-haystack kernels stage leading wide records
+size_t plan_smem(const dach_dev* d, ScanParams& P, bool v1, bool std3, int threads, int ctas_per_sm, int queue_sets) {
+    const size_t smem_budget = std::min<size_t>(d->smem_optin, 226 * 1024) / ctas_per_sm - (ctas_per_sm > 1 ? 1024 : 0);
+    size_t smem;
+    if (v1) {
+        const size_t queues = (size_t)LANE_Q * threads * sizeof(QEntry) * queue_sets;
+        // StdMachine3: the front of the hot region next to the queues (whole 256-slot blocks)
+        uint64_t want = 0;
+        if (std3 && d->opt_hot_entries != 0 && smem_budget > queues + 512) {
+            want = std::min<uint64_t>(d->hot_slots, (smem_budget - queues - 512) / 16);
+            if (d->opt_hot_entries > 0) want = std::min<uint64_t>(want, (uint64_t)d->opt_hot_entries);
+            want &= ~uint64_t(255);
+        }
+        smem = (size_t)want * 16 + queues;
+        if (d->opt_smem_pad_kib > 0) smem = std::min<size_t>(smem + ((size_t)d->opt_smem_pad_kib << 10), smem_budget);
+        P.hot_n = 0;
+        P.hot_entries = (uint32_t)want;
+    } else {
+        uint64_t hot = smem_budget > kRootBytes ? (smem_budget - kRootBytes) / 16 : 0;
+        if (d->opt_hot_records >= 0) hot = std::min<uint64_t>(hot, (uint64_t)d->opt_hot_records);
+        hot = std::min<uint64_t>(hot, d->n_slots);
+        P.hot_n = (uint32_t)hot;
+        smem = kRootBytes + (size_t)hot * 16;
+    }
+    return smem;
+}
+
+// segment table: counts per haystack -> first item per haystack (W.seg_first) -> (haystack, begin) per item
+void enqueue_seg_table(dach_dev* d, Workspace& W, const uint64_t* d_offs, uint64_t n, uint32_t seg_len, uint32_t seg_from,
+                       ScanParams& P, cudaStream_t st) {
+    unsigned long long* tiles = static_cast<unsigned long long*>(W.tiles.p);
+    unsigned long long* seg_first = static_cast<unsigned long long*>(W.seg_first.p);
+    const unsigned hb = (unsigned)((n + 255) / 256), hb1 = (unsigned)((n + 1 + 255) / 256);
+    const uint64_t nt = (n + kScanTile - 1) / kScanTile;
+    uint32_t* nseg = static_cast<uint32_t*>(W.nseg.p);
+    k_seg_count<<<hb, 256, 0, st>>>(d_offs, n, seg_len, seg_from, nseg, P.ctrl);
+    k_offsets_tile_sums<false><<<(unsigned)nt, kScanThreads, 0, st>>>(nseg, n, tiles);
+    k_offsets_scan_tiles<<<1, kScanThreads, 0, st>>>(tiles, nt);
+    k_offsets_apply<false><<<(unsigned)nt, kScanThreads, 0, st>>>(nseg, n, tiles, seg_first);
+    k_seg_fill<<<hb1, 256, 0, st>>>(seg_first, nseg, n, seg_len, static_cast<uint32_t*>(W.item_hay.p),
+                                    static_cast<uint32_t*>(W.item_beg.p), static_cast<unsigned long long*>(W.n_items_dev.p));
+    d->launches += 5;
+    P.item_hay = static_cast<const uint32_t*>(W.item_hay.p);
+    P.item_beg = static_cast<const uint32_t*>(W.item_beg.p);
+    P.n_items_dev = static_cast<const unsigned long long*>(W.n_items_dev.p);
+    P.seg_len = seg_len;
+    P.seg_from = seg_from;
+    P.warm = d->max_pattern_len ? d->max_pattern_len - 1 : 0;
 }
 
 // ---- phase 1: items, scan kernel, per-item offsets, block index.  No synchronisation. ------------------
@@ -1087,78 +1307,21 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
                 !ensure(W.item_beg, n_items_max * 4) || !ensure(W.n_items_dev, 8)))
         return DACH_CUDA_ERROR;
 
-    ScanParams P;
-    memset(&P, 0, sizeof(P));
-    P.rec = d->d_rec;
-    P.outputs = d->d_outputs;
-    P.root_table = d->d_root;
-    P.crec = d->d_crec;
-    P.opos_tab = d->d_opos;
-    P.root_base = d->root_base;
-    P.mapper = d->d_mapper;
-    P.mapper_len = d->mapper_len;
-    P.n_slots = d->n_slots;
-    P.id_in = d->d_id_in;
-    P.id_out = d->d_id_out;
-    P.root_opos = d->root_opos;
-    P.text = d_text;
-    P.text_lo = text_lo;
-    P.text_end = text_end;
-    P.offs = d_offs;
-    P.n_items = n;
+    ScanParams P = image_params(d, d_text, text_lo, text_end, d_offs, n);
     P.counts = static_cast<uint32_t*>(W.counts.p);
     P.pool = static_cast<uint32_t*>(W.pool.p);
     P.pool_blocks = pool_blocks;
     P.ctrl = static_cast<ScanCtrl*>(W.ctrl.p);
     P.state_io = d_state_io;
-
-    const size_t smem_budget = std::min<size_t>(d->smem_optin, 226 * 1024) / ctas_per_sm - (ctas_per_sm > 1 ? 1024 : 0);
-    size_t smem;
-    if (v1) {
-        const size_t queues = (size_t)LANE_Q * threads * sizeof(QEntry) * (duo ? 2 : 1);
-        // StdMachine3: the front of the hot region next to the queues (whole 256-slot blocks)
-        uint64_t want = 0;
-        if (std3 && d->opt_hot_entries != 0 && smem_budget > queues + 512) {
-            want = std::min<uint64_t>(d->hot_slots, (smem_budget - queues - 512) / 16);
-            if (d->opt_hot_entries > 0) want = std::min<uint64_t>(want, (uint64_t)d->opt_hot_entries);
-            want &= ~uint64_t(255);
-        }
-        smem = (size_t)want * 16 + queues;
-        if (d->opt_smem_pad_kib > 0) smem = std::min<size_t>(smem + ((size_t)d->opt_smem_pad_kib << 10), smem_budget);
-        P.hot_n = 0;
-        P.hot_entries = (uint32_t)want;
-    } else {
-        uint64_t hot = smem_budget > kRootBytes ? (smem_budget - kRootBytes) / 16 : 0;
-        if (d->opt_hot_records >= 0) hot = std::min<uint64_t>(hot, (uint64_t)d->opt_hot_records);
-        hot = std::min<uint64_t>(hot, d->n_slots);
-        P.hot_n = (uint32_t)hot;
-        smem = kRootBytes + (size_t)hot * 16;
-    }
+    const size_t smem = plan_smem(d, P, v1, std3, threads, ctas_per_sm, duo ? 2 : 1);
 
     unsigned long long* tiles = static_cast<unsigned long long*>(W.tiles.p);
-    unsigned long long* seg_first = static_cast<unsigned long long*>(W.seg_first.p);
     unsigned long long* item_offs = static_cast<unsigned long long*>(W.item_offs.p);
     k_check_offsets<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_offs, n, (uint64_t)(text_end - d_text), P.ctrl);
     ++d->launches;
     if (seg) {
-        // segment table: counts per haystack -> first item per haystack -> (haystack, begin) per item
-        const unsigned hb = (unsigned)((n + 255) / 256), hb1 = (unsigned)((n + 1 + 255) / 256);
-        const uint64_t nt = (n + kScanTile - 1) / kScanTile;
-        uint32_t* nseg = static_cast<uint32_t*>(W.nseg.p);
         cudaMemsetAsync(W.counts.p, 0, n_items_max * 4, st);  // items past the real count stay empty
-        k_seg_count<<<hb, 256, 0, st>>>(d_offs, n, seg_len, seg_from, nseg, P.ctrl);
-        k_offsets_tile_sums<false><<<(unsigned)nt, kScanThreads, 0, st>>>(nseg, n, tiles);
-        k_offsets_scan_tiles<<<1, kScanThreads, 0, st>>>(tiles, nt);
-        k_offsets_apply<false><<<(unsigned)nt, kScanThreads, 0, st>>>(nseg, n, tiles, seg_first);
-        k_seg_fill<<<hb1, 256, 0, st>>>(seg_first, nseg, n, seg_len, static_cast<uint32_t*>(W.item_hay.p),
-                                        static_cast<uint32_t*>(W.item_beg.p), static_cast<unsigned long long*>(W.n_items_dev.p));
-        d->launches += 5;
-        P.item_hay = static_cast<const uint32_t*>(W.item_hay.p);
-        P.item_beg = static_cast<const uint32_t*>(W.item_beg.p);
-        P.n_items_dev = static_cast<const unsigned long long*>(W.n_items_dev.p);
-        P.seg_len = seg_len;
-        P.seg_from = seg_from;
-        P.warm = d->max_pattern_len ? d->max_pattern_len - 1 : 0;
+        enqueue_seg_table(d, W, d_offs, n, seg_len, seg_from, P, st);
     }
     cudaEventRecord(W.ev[3], st);
     if (!cuda_ok(cw_machine   ? launch_cw(mode, P, grid, std::min(threads, 1024), smem, st)
@@ -1300,23 +1463,9 @@ int scan_locked(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, cons
     return finish_scan(d, W, out_cap, needed);
 }
 
-int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n,
-                         dach_match* out, uint64_t out_cap, uint64_t* out_offs, uint64_t* needed) {
-    if (!d || !offs || !out_offs || (out_cap && !out)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    int rc = check_mode(d, mode);
-    if (rc) return rc;
-    std::lock_guard<std::mutex> lk(d->mu);
-    DeviceGuard g(d->device);
-    if (!g.ok) return DACH_CUDA_ERROR;
-    d->last_h2d = d->last_d2h = 0;
-    if (n == 0) {
-        out_offs[0] = 0;
-        if (needed) *needed = 0;
-        return DACH_OK;
-    }
+double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+int check_host_offsets(const uint64_t* offs, uint64_t n) {
     for (uint64_t i = 0; i < n; ++i) {
         if (offs[i + 1] < offs[i]) {
             set_error("haystack offsets must be ascending");
@@ -1327,15 +1476,17 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
             return DACH_INVALID_ARGUMENT;
         }
     }
-    // whatever is still queued on the slots' streams reads the caller's text or writes the caller's buffers:
-    // no exit from here on may leave it in flight
-    struct Drain {
-        dach_dev* d;
-        ~Drain() {
-            for (Workspace& w : d->slot)
-                if (w.stream) cudaStreamSynchronize(w.stream);
-        }
-    } drain_on_exit{d};
+    return DACH_OK;
+}
+
+struct Slice {
+    uint64_t first, last;  // haystacks [first, last)
+    uint64_t base;         // matches before this slice
+    uint64_t total;
+};
+
+// The slices a host-buffer batch (n > 0) goes to the device in: whole haystacks; `mode` is the iterator the device runs.
+std::vector<Slice> cut_slices(const dach_dev* d, int mode, const uint64_t* offs, uint64_t n) {
     // Slices of ~slice_mib MiB of text, three in flight: while slice k is scanned, slice k+1 is
     // on its way to the device and the matches of slice k-1 are on their way back.
     uint64_t slice_bytes = (uint64_t)std::max<int64_t>(d->opt_slice_mib, 1) << 20;
@@ -1346,11 +1497,6 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
         const uint64_t lanes = (uint64_t)d->sm_count * 1024, avg = (offs[n] - offs[0]) / n + 1;
         if (!segmentable) slice_bytes = std::min<uint64_t>(std::max(slice_bytes, lanes * avg), 1ull << 30);
     }
-    struct Slice {
-        uint64_t first, last;  // haystacks [first, last)
-        uint64_t base;         // matches before this slice
-        uint64_t total;
-    };
     std::vector<Slice> slices;
     // Slice sizes ramp up at the head of the batch and down at its tail (1/8, 1/4, 1/2, 1, ..., 1/2, 1/4,
     // 1/8 of slice_bytes): nothing can be scanned before the first upload lands and nothing overlaps the
@@ -1380,6 +1526,75 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
         slices.push_back({i, j, 0, 0});
         i = j;
     }
+    return slices;
+}
+
+// Uploads haystacks [first, last) of a host batch into W's text and offsets buffers on W's stream once the slot's
+// previous work is done (the wait is added to *t_reuse).
+bool slice_h2d(dach_dev* d, Workspace& W, const uint8_t* text, const uint64_t* offs, uint64_t first, uint64_t last, double* t_reuse) {
+    const uint64_t tb = offs[last] - offs[first], ns = last - first;
+    const double t0 = now_ms();
+    if (!cuda_ok(cudaStreamSynchronize(W.stream), "slot reuse")) return false;
+    *t_reuse += now_ms() - t0;
+    if (!ensure(W.text, tb + 32) || !ensure(W.offs, (ns + 1) * 8) || !ensure(W.out_offs, (ns + 1) * 8)) return false;
+    if (tb && !cuda_ok(cudaMemcpyAsync(W.text.p, text + offs[first], tb, cudaMemcpyHostToDevice, W.stream), "H2D text"))
+        return false;
+    // The offsets go through a pinned staging buffer: an async copy from pageable memory first waits
+    // for everything queued in the stream (here: the 64 MiB text upload) and blocks the host meanwhile,
+    // which starves the whole pipeline.  (The slot's stream was synchronised above, so the buffer is free.)
+    const void* offs_src = offs + first;
+    const size_t ob = (ns + 1) * 8;
+    if (W.offs_stage_bytes < ob) {
+        if (W.offs_stage) cudaFreeHost(W.offs_stage);
+        W.offs_stage = nullptr;
+        W.offs_stage_bytes = 0;
+        void* q = nullptr;
+        if (cudaMallocHost(&q, ob + ob / 2) == cudaSuccess) {
+            W.offs_stage = q;
+            W.offs_stage_bytes = ob + ob / 2;
+        } else {
+            cudaGetLastError();  // no staging: copy from the caller's memory directly
+        }
+    }
+    if (W.offs_stage) {
+        memcpy(W.offs_stage, offs_src, ob);
+        offs_src = W.offs_stage;
+    }
+    if (!cuda_ok(cudaMemcpyAsync(W.offs.p, offs_src, ob, cudaMemcpyHostToDevice, W.stream), "H2D offsets"))
+        return false;
+    d->last_h2d += tb + (ns + 1) * 8;
+    return true;
+}
+
+int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n,
+                         dach_match* out, uint64_t out_cap, uint64_t* out_offs, uint64_t* needed) {
+    if (!d || !offs || !out_offs || (out_cap && !out)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    int rc = check_mode(d, mode);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(d->mu);
+    DeviceGuard g(d->device);
+    if (!g.ok) return DACH_CUDA_ERROR;
+    d->last_h2d = d->last_d2h = 0;
+    if (n == 0) {
+        out_offs[0] = 0;
+        if (needed) *needed = 0;
+        return DACH_OK;
+    }
+    rc = check_host_offsets(offs, n);
+    if (rc) return rc;
+    // whatever is still queued on the slots' streams reads the caller's text or writes the caller's buffers:
+    // no exit from here on may leave it in flight
+    struct Drain {
+        dach_dev* d;
+        ~Drain() {
+            for (Workspace& w : d->slot)
+                if (w.stream) cudaStreamSynchronize(w.stream);
+        }
+    } drain_on_exit{d};
+    std::vector<Slice> slices = cut_slices(d, mode, offs, n);
     for (Workspace& w : d->slot)
         if (!w.init(true)) return DACH_CUDA_ERROR;
     // every slot's previous work must be finished before its buffers are reused
@@ -1387,43 +1602,10 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
     uint64_t base = 0;
     const bool trace = getenv("DACH_DEBUG") != nullptr;
     double t_reuse = 0, t_scan = 0, t_final = 0, gpu_ms = 0;
-    auto now = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
+    auto now = now_ms;
     const double t_begin = now();
     auto issue_h2d = [&](size_t k) -> bool {
-        Workspace& W = d->slot[k % dach_dev::kSlots];
-        const Slice& s = slices[k];
-        const uint64_t tb = offs[s.last] - offs[s.first], ns = s.last - s.first;
-        const double t0 = now();
-        if (!cuda_ok(cudaStreamSynchronize(W.stream), "slot reuse")) return false;
-        t_reuse += now() - t0;
-        if (!ensure(W.text, tb + 32) || !ensure(W.offs, (ns + 1) * 8) || !ensure(W.out_offs, (ns + 1) * 8)) return false;
-        if (tb && !cuda_ok(cudaMemcpyAsync(W.text.p, text + offs[s.first], tb, cudaMemcpyHostToDevice, W.stream), "H2D text"))
-            return false;
-        // The offsets go through a pinned staging buffer: an async copy from pageable memory first waits
-        // for everything queued in the stream (here: the 64 MiB text upload) and blocks the host meanwhile,
-        // which starves the whole pipeline.  (The slot's stream was synchronised above, so the buffer is free.)
-        const void* offs_src = offs + s.first;
-        const size_t ob = (ns + 1) * 8;
-        if (W.offs_stage_bytes < ob) {
-            if (W.offs_stage) cudaFreeHost(W.offs_stage);
-            W.offs_stage = nullptr;
-            W.offs_stage_bytes = 0;
-            void* q = nullptr;
-            if (cudaMallocHost(&q, ob + ob / 2) == cudaSuccess) {
-                W.offs_stage = q;
-                W.offs_stage_bytes = ob + ob / 2;
-            } else {
-                cudaGetLastError();  // no staging: copy from the caller's memory directly
-            }
-        }
-        if (W.offs_stage) {
-            memcpy(W.offs_stage, offs_src, ob);
-            offs_src = W.offs_stage;
-        }
-        if (!cuda_ok(cudaMemcpyAsync(W.offs.p, offs_src, ob, cudaMemcpyHostToDevice, W.stream), "H2D offsets"))
-            return false;
-        d->last_h2d += tb + (ns + 1) * 8;
-        return true;
+        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
     };
     // The copy engine must never wait for the host: the host blocks in scan_locked() until slice k is
     // scanned, so the uploads of the next TWO slices are queued before that (with one slice ahead the
@@ -1486,6 +1668,173 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
         const uint64_t hi = (k + 1 == slices.size()) ? s.last + 1 : s.last;
         for (uint64_t i = s.first; i < hi; ++i) out_offs[i] += s.base;
     }
+    return DACH_OK;
+}
+
+// ---- COUNT / FIRST: the scan of a batch and its per-haystack results on one stream.  No synchronisation. ----------
+// rk = RK_COUNT: d_counts (n x u64); RK_FIRST: d_first (n tuples), d_found (n x u8).  The total (matches, or haystacks
+// with a match) lands in W.pinned->total_rk once W.ev_placed has completed.  No block pool, no offsets, no gather:
+// options kernel = 1, 2, 4 run StdMachine3 here (kernel = 0: the lane-per-haystack kernels).
+int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
+               uint64_t text_bytes, const uint64_t* d_offs, uint64_t n, uint64_t* d_counts, dach_match* d_first, uint8_t* d_found,
+               cudaStream_t st) {
+    if (n > 0xfffffff0ull) {
+        set_error("too many haystacks in one batch (max 2^32-16)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    if (W.job_open) cudaStreamWaitEvent(st, W.ev_placed, 0);
+    if (!ensure(W.ctrl, sizeof(ScanCtrl)) || !ensure(W.total_rk, 8)) return DACH_CUDA_ERROR;
+    if (!cuda_ok(cudaMemsetAsync(W.ctrl.p, 0, sizeof(ScanCtrl), st), "memset ctrl") ||
+        !cuda_ok(cudaMemsetAsync(W.total_rk.p, 0, 8, st), "memset total"))
+        return DACH_CUDA_ERROR;
+    cudaEventRecord(W.ev[0], st);
+    cudaEventRecord(W.ev[3], st);
+    unsigned long long* total = static_cast<unsigned long long*>(W.total_rk.p);
+    if (n > 0) {
+        int threads = (int)std::min<int64_t>(std::max<int64_t>(d->opt_threads, 32), kMaxThreads);
+        threads = (threads / 32) * 32;
+        const int ctas_per_sm = (int)std::min<int64_t>(std::max<int64_t>(d->opt_ctas_per_sm, 1), 2048 / threads);
+        const int free_sms = (int)std::min<int64_t>(std::max<int64_t>(d->opt_reserve_sms, 0), d->sm_count - 1);
+        const int grid = (d->sm_count - free_sms) * ctas_per_sm;
+        // the first event of a haystack is the same for all three Standard iterators: FIRST runs find_overlapping
+        const int mmode = (rk == RK_FIRST && mode != M_LEFTMOST) ? M_OVERLAPPING : mode;
+        const bool v1 = d->opt_kernel >= 1 && d->d_crec && !(mmode == M_FIND && d->root_opos != 0);
+        const bool cw_machine = v1 && d->charwise;
+        const bool lm_machine = v1 && !d->charwise && mmode == M_LEFTMOST;
+        const bool std3 = v1 && !d->charwise && mmode != M_LEFTMOST && d->root_base != 0;
+        const bool machine = cw_machine || lm_machine || std3;
+        // segments as in enqueue_scan (no tail-only cutting)
+        bool seg = std3 && (mmode == M_OVERLAPPING || mmode == M_NO_SUFFIX) && d->opt_seg_len >= 0 && d->segmentable;
+        uint32_t seg_len = 0;
+        uint64_t n_items_max = n;
+        if (seg) {
+            const uint64_t lanes = (uint64_t)grid * threads;
+            const uint64_t warm = d->max_pattern_len ? d->max_pattern_len - 1 : 0;
+            uint64_t want = d->opt_seg_len > 0 ? (uint64_t)d->opt_seg_len : std::max(text_bytes / (2 * lanes) + 1, std::max<uint64_t>(256, 8 * warm));
+            want = (want + 255) & ~uint64_t(255);
+            if (want >= text_bytes || want >= (1ull << 31)) {
+                seg = false;
+            } else {
+                seg_len = (uint32_t)want;
+                n_items_max = n + text_bytes / seg_len + 1;
+                if (n_items_max > 0xfffffff0ull) seg = false, n_items_max = n;
+            }
+        }
+        const uint64_t n_tiles = (n + kScanTile - 1) / kScanTile;
+        if (!ensure(W.items_rk, n_items_max * (rk == RK_FIRST ? 16 : 8))) return DACH_CUDA_ERROR;
+        if (seg && (!ensure(W.tiles, n_tiles * 8) || !ensure(W.nseg, n * 4) || !ensure(W.seg_first, (n + 1) * 8) ||
+                    !ensure(W.item_hay, n_items_max * 4) || !ensure(W.item_beg, n_items_max * 4) || !ensure(W.n_items_dev, 8)))
+            return DACH_CUDA_ERROR;
+        ScanParams P = image_params(d, d_text, text_lo, text_end, d_offs, n);
+        P.ctrl = static_cast<ScanCtrl*>(W.ctrl.p);
+        P.item_count = static_cast<unsigned long long*>(W.items_rk.p);
+        P.item_first = static_cast<uint4*>(W.items_rk.p);
+        const size_t smem = plan_smem(d, P, machine, std3, threads, ctas_per_sm, 1);
+        k_check_offsets<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_offs, n, (uint64_t)(text_end - d_text), P.ctrl);
+        ++d->launches;
+        if (seg) enqueue_seg_table(d, W, d_offs, n, seg_len, 0, P, st);
+        cudaEventRecord(W.ev[3], st);
+        const int which = std3 ? 3 : machine ? 1 : 0;
+        const int t = machine ? std::min(threads, 1024) : threads;
+        if (!cuda_ok(rk == RK_COUNT ? launch_rk<RK_COUNT>(which, d->charwise, mmode, P, grid, t, smem, st)
+                                    : launch_rk<RK_FIRST>(which, d->charwise, mmode, P, grid, t, smem, st),
+                     "k_scan launch"))
+            return DACH_CUDA_ERROR;
+        cudaEventRecord(W.ev[1], st);
+        const unsigned long long* seg_first = seg ? static_cast<const unsigned long long*>(W.seg_first.p) : nullptr;
+        if (rk == RK_COUNT)
+            k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(d_counts), total);
+        else
+            k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(d_first), d_found, total);
+        d->launches += 2;
+        if (!cuda_ok(cudaGetLastError(), "kernel launch")) return DACH_CUDA_ERROR;
+    } else {
+        cudaEventRecord(W.ev[1], st);
+    }
+    cudaEventRecord(W.ev[2], st);
+    cudaMemcpyAsync(&W.pinned->total_rk, total, 8, cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(&W.pinned->ctrl, W.ctrl.p, sizeof(ScanCtrl), cudaMemcpyDeviceToHost, st);
+    cudaEventRecord(W.ev_placed, st);
+    return DACH_OK;
+}
+
+// wait for enqueue_rk's work, report
+int finish_rk(dach_dev* d, Workspace& W, uint64_t* total) {
+    if (!cuda_ok(cudaEventSynchronize(W.ev_placed), "scan pipeline")) return DACH_CUDA_ERROR;
+    float ms = 0;
+    if (cudaEventElapsedTime(&ms, W.ev[3], W.ev[1]) == cudaSuccess) d->last_scan_ms = ms;
+    if (cudaEventElapsedTime(&ms, W.ev[0], W.ev[2]) == cudaSuccess) d->last_total_ms = ms;
+    if (W.pinned->ctrl.bad_offsets) {
+        set_error("haystack offsets must be ascending and inside text_bytes, and no haystack may reach 4 GiB (match positions are u32)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    if (total) *total = W.pinned->total_rk;
+    return DACH_OK;
+}
+
+// COUNT / FIRST of a host-buffer batch: the slices of dach_scan_batch_host; only the per-haystack results come back
+int rk_batch_host_impl(dach_dev* d, int rk, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* counts,
+                       dach_match* first, uint8_t* found, uint64_t* total) {
+    if (!d || !offs || (n && (rk == RK_COUNT ? !counts : (!first || !found)))) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    int rc = check_mode(d, mode);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(d->mu);
+    DeviceGuard g(d->device);
+    if (!g.ok) return DACH_CUDA_ERROR;
+    d->last_h2d = d->last_d2h = 0;
+    if (total) *total = 0;
+    if (n == 0) return DACH_OK;
+    rc = check_host_offsets(offs, n);
+    if (rc) return rc;
+    struct Drain {  // no exit may leave copies of the caller's buffers in flight
+        dach_dev* d;
+        ~Drain() {
+            for (Workspace& w : d->slot)
+                if (w.stream) cudaStreamSynchronize(w.stream);
+        }
+    } drain_on_exit{d};
+    const std::vector<Slice> slices = cut_slices(d, (rk == RK_FIRST && mode != M_LEFTMOST) ? M_OVERLAPPING : mode, offs, n);
+    for (Workspace& w : d->slot)
+        if (!w.init(true)) return DACH_CUDA_ERROR;
+    double t_reuse = 0;
+    auto issue_h2d = [&](size_t k) -> bool {
+        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
+    };
+    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
+    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
+    uint64_t sum = 0;
+    for (size_t k = 0; k < slices.size(); ++k) {
+        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
+        Workspace& W = d->slot[k % dach_dev::kSlots];
+        const Slice& s = slices[k];
+        const uint64_t tb = offs[s.last] - offs[s.first], ns = s.last - s.first;
+        if (!ensure(W.out, ns * sizeof(dach_match) + 16)) return DACH_CUDA_ERROR;
+        const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
+        // COUNT: counts in W.out; FIRST: tuples in W.out, found flags in W.out_offs
+        rc = enqueue_rk(d, W, rk, mode, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb, tb,
+                        static_cast<const uint64_t*>(W.offs.p), ns, static_cast<uint64_t*>(W.out.p), static_cast<dach_match*>(W.out.p),
+                        static_cast<uint8_t*>(W.out_offs.p), W.stream);
+        uint64_t t = 0;
+        if (!rc) rc = finish_rk(d, W, &t);
+        if (rc) return rc;
+        sum += t;
+        if (rk == RK_COUNT) {
+            if (!cuda_ok(cudaMemcpyAsync(counts + s.first, W.out.p, ns * 8, cudaMemcpyDeviceToHost, W.stream), "D2H counts"))
+                return DACH_CUDA_ERROR;
+            d->last_d2h += ns * 8;
+        } else {
+            if (!cuda_ok(cudaMemcpyAsync(first + s.first, W.out.p, ns * sizeof(dach_match), cudaMemcpyDeviceToHost, W.stream), "D2H first") ||
+                !cuda_ok(cudaMemcpyAsync(found + s.first, W.out_offs.p, ns, cudaMemcpyDeviceToHost, W.stream), "D2H found"))
+                return DACH_CUDA_ERROR;
+            d->last_d2h += ns * (sizeof(dach_match) + 1);
+        }
+    }
+    for (Workspace& w : d->slot)
+        if (!cuda_ok(cudaStreamSynchronize(w.stream), "D2H")) return DACH_CUDA_ERROR;
+    if (total) *total = sum;
     return DACH_OK;
 }
 
@@ -1642,6 +1991,51 @@ int dach_dev_scan_stream(dach_dev* d, int mode, const uint8_t* d_text, const uin
 int dach_scan_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n,
                          dach_match* out, uint64_t out_cap, uint64_t* out_offs, uint64_t* needed) {
     return guarded([&]() -> int { return scan_batch_host_impl(d, mode, text, offs, n, out, out_cap, out_offs, needed); });
+}
+
+int dach_dev_count_batch(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                         uint64_t* d_counts, uint64_t* total, void* stream) {
+    if (!d || !d_offs || (n && !d_counts)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    const int rc = check_mode(d, mode);
+    if (rc) return rc;
+    return guarded([&]() -> int {
+        std::lock_guard<std::mutex> lk(d->mu);
+        DeviceGuard g(d->device);
+        if (!g.ok) return DACH_CUDA_ERROR;
+        const int r = enqueue_rk(d, d->ws, RK_COUNT, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, d_counts, nullptr,
+                                 nullptr, static_cast<cudaStream_t>(stream));
+        return r ? r : finish_rk(d, d->ws, total);
+    });
+}
+
+int dach_count_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* counts, uint64_t* total) {
+    return guarded([&]() -> int { return rk_batch_host_impl(d, RK_COUNT, mode, text, offs, n, counts, nullptr, nullptr, total); });
+}
+
+int dach_dev_first_batch(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                         dach_match* d_first, uint8_t* d_found, uint64_t* n_found, void* stream) {
+    if (!d || !d_offs || (n && (!d_first || !d_found))) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    const int rc = check_mode(d, mode);
+    if (rc) return rc;
+    return guarded([&]() -> int {
+        std::lock_guard<std::mutex> lk(d->mu);
+        DeviceGuard g(d->device);
+        if (!g.ok) return DACH_CUDA_ERROR;
+        const int r = enqueue_rk(d, d->ws, RK_FIRST, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, nullptr, d_first,
+                                 d_found, static_cast<cudaStream_t>(stream));
+        return r ? r : finish_rk(d, d->ws, n_found);
+    });
+}
+
+int dach_first_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, dach_match* first, uint8_t* found,
+                          uint64_t* n_found) {
+    return guarded([&]() -> int { return rk_batch_host_impl(d, RK_FIRST, mode, text, offs, n, nullptr, first, found, n_found); });
 }
 
 // ---- asynchronous jobs ------------------------------------------------------------------------------

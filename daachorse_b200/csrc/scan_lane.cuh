@@ -16,6 +16,8 @@
 //   - StdMachine3  the default (kernel=3): no probe-state flags, one stop bit, cursor = address word, records from
 //                  the hot-first image (optionally its front from shared memory); probe / resolve are separate so
 //                  that k_scan_duo can keep two fetches in flight; serves stream chunks
+//   - SinkOps      COUNT / FIRST on StdMachine3, LmMachine, CwMachine: their drain() / begin_item() for the
+//                  other result kinds (sinks: Emitter, CountSink, FirstSink)
 //
 // Device image (built by dev_image.cpp from the validated host automaton):
 //   wide bytewise record  uint4 {base, efail, fbase, opos<<8 | check}      16 B / slot
@@ -29,11 +31,15 @@
 //               so a second miss goes straight to the dense root row (slots are < 2^31)
 //   wide charwise record  uint4 {base, check(parent), fail, output_pos}    src/charwise.rs:1096-1101
 //   compact records (lane machines, at most 2^24 slots): described above each machine
-//   output           uint4 {value, length, parent, 0}                      src/lib.rs:213-218
+//   output           uint4 {value, length, parent, chain}                  src/lib.rs:213-218
+//       chain   length of the list that starts at this record (1 + chain of the parent): COUNT adds it per
+//               find_overlapping event instead of walking the list
 //   root table       256 x u32                                             src/bytewise.rs:1040-1056
 #pragma once
 
 #include <stdint.h>
+
+#include <type_traits>
 
 #if defined(__CUDACC__)
 #define DACH_HD __host__ __device__ __forceinline__
@@ -132,7 +138,15 @@ struct ScanParams {
     uint32_t* pool;
     uint32_t pool_blocks;
     ScanCtrl* ctrl;
+    // results of the other result kinds (CountSink / FirstSink), per item
+    unsigned long long* item_count;
+    uint4* item_first;  // {start, end, value, found}
 };
+
+// What a scan produces (compile time): every match (Emitter), the number of matches (CountSink), or the first
+// match and whether there is one (FirstSink).  The lane machines and the lane-per-haystack loops are the same
+// for all three; the sink and, for FIRST, the stop rule differ.
+constexpr int RK_MATCHES = 0, RK_COUNT = 1, RK_FIRST = 2;
 
 // L2 eviction policies (64-bit descriptors made once per device by k_make_policies, dev_scan.cu):
 //   [0] automaton image (records, output_pos, outputs, mapper): evict_last -- the scan is latency-bound on
@@ -249,6 +263,7 @@ struct TextWin {
 
 // ---- match emission --------------------------------------------------------------------
 struct Emitter {
+    static constexpr int KIND = RK_MATCHES;
     uint32_t* blk;   // current block (nullptr when the pool is exhausted or nothing emitted yet)
     uint32_t fill;   // matches in the current block
     uint32_t count;  // matches of the current item
@@ -278,7 +293,47 @@ struct Emitter {
         ++count;
     }
     DACH_HD void finish(const ScanParams& P) { P.counts[item] = count; }
+    DACH_HD bool stopped() const { return false; }
 };
+
+// COUNT: matches of the current item, 64-bit (overlapping lists make more than 2^32 matches on one haystack reachable)
+struct CountSink {
+    static constexpr int KIND = RK_COUNT;
+    unsigned long long count;
+    uint32_t item;
+    DACH_HD void begin(uint32_t item_id) {
+        count = 0;
+        item = item_id;
+    }
+    DACH_HD void emit(const ScanParams&, uint32_t, uint32_t, uint32_t) { ++count; }
+    DACH_HD void finish(const ScanParams& P) { P.item_count[item] = count; }
+    DACH_HD bool stopped() const { return false; }
+};
+
+// FIRST: the first match of the current item; the scan of the item stops once it has one
+struct FirstSink {
+    static constexpr int KIND = RK_FIRST;
+    uint32_t start, end, value, found, item;
+    DACH_HD void begin(uint32_t item_id) {
+        start = end = value = 0xffffffffu;
+        found = 0;
+        item = item_id;
+    }
+    DACH_HD void emit(const ScanParams&, uint32_t s, uint32_t e, uint32_t v) {
+        if (!found) start = s, end = e, value = v, found = 1;
+    }
+    DACH_HD void finish(const ScanParams& P) {
+        uint4 r;
+        r.x = start, r.y = end, r.z = value, r.w = found;
+        P.item_first[item] = r;
+    }
+    DACH_HD bool stopped() const { return found != 0; }
+};
+
+// the chain word of output record `opos` (1-based): how many patterns the list from there holds
+DACH_HD uint32_t chain_len(const ScanParams& P, uint32_t opos) {
+    return ld_u32(reinterpret_cast<const uint32_t*>(P.outputs + (opos - 1)) + 3);
+}
 
 // Walk a merged output list from `opos` (1-based, 0 = end), emitting every pattern ending
 // at `end` (src/bytewise/iter.rs:134-148).
@@ -292,6 +347,19 @@ DACH_HD void emit_chain(const ScanParams& P, Emitter& E, uint32_t opos, uint32_t
 DACH_HD void emit_head(const ScanParams& P, Emitter& E, uint32_t opos, uint32_t end) {
     const uint4 o = ld_u4(P.outputs + (opos - 1));
     E.emit(P, end - o.y, end, o.x);
+}
+// COUNT: one loaded word per list, no walk; a head is one match
+DACH_HD void emit_chain(const ScanParams& P, CountSink& E, uint32_t opos, uint32_t) {
+    if (opos != 0) E.count += chain_len(P, opos);
+}
+DACH_HD void emit_head(const ScanParams&, CountSink& E, uint32_t, uint32_t) { ++E.count; }
+// FIRST: a list's first match is its head
+DACH_HD void emit_head(const ScanParams& P, FirstSink& E, uint32_t opos, uint32_t end) {
+    const uint4 o = ld_u4(P.outputs + (opos - 1));
+    E.emit(P, end - o.y, end, o.x);
+}
+DACH_HD void emit_chain(const ScanParams& P, FirstSink& E, uint32_t opos, uint32_t end) {
+    if (opos != 0) emit_head(P, E, opos, end);
 }
 
 // ---- record access: leading `hot_n` records come from shared memory --------------------
@@ -410,8 +478,8 @@ DACH_HD uint32_t cw_step(const ScanParams& P, const RecView& V, uint32_t s, uint
 // ---- one haystack, Standard modes --------------------------------------------------------
 // FindIterator / FindOverlappingIterator / FindOverlappingNoSuffixIterator
 // (src/bytewise/iter.rs:58-113, 133-176, 195-243; src/charwise/iter.rs:115-170, 190-235, 254-302)
-template <bool CHARWISE, int MODE>
-DACH_HD void scan_standard(const ScanParams& P, const RecView& V, TextWin& T, Emitter& E, uint32_t len) {
+template <bool CHARWISE, int MODE, class SINK>
+DACH_HD void scan_standard(const ScanParams& P, const RecView& V, TextWin& T, SINK& E, uint32_t len) {
     const uint32_t root_opos = P.root_opos;
     uint4 root_rec = {0, 0, 0, 0};
     if (CHARWISE) root_rec = V.get(D_ROOT);
@@ -426,6 +494,7 @@ DACH_HD void scan_standard(const ScanParams& P, const RecView& V, TextWin& T, Em
         E.emit(P, 0, 0, v);
         uint32_t pos = 0;
         while (pos < len) {
+            if constexpr (SINK::KIND == RK_FIRST) return;  // the first match is (0, 0)
             if (CHARWISE)
                 (void)utf8_at(T, pos);
             else
@@ -438,6 +507,9 @@ DACH_HD void scan_standard(const ScanParams& P, const RecView& V, TextWin& T, Em
     uint4 r = root_rec;
     uint32_t pos = 0;
     while (pos < len) {
+        if constexpr (SINK::KIND == RK_FIRST) {
+            if (E.stopped()) return;
+        }
         if (CHARWISE) {
             const uint32_t cp = utf8_at(T, pos);
             if (s == D_ROOT) r = root_rec;
@@ -469,8 +541,8 @@ DACH_HD void scan_standard(const ScanParams& P, const RecView& V, TextWin& T, Em
 // LeftmostFindIterator (src/bytewise/iter.rs:272-340; src/charwise/iter.rs:328-399).  The
 // iterator fields (pos, init_output_pos, skip_empty) persist across next() calls; one turn of
 // the outer loop is one next().
-template <bool CHARWISE>
-DACH_HD void scan_leftmost(const ScanParams& P, const RecView& V, TextWin& T, Emitter& E, uint32_t len) {
+template <bool CHARWISE, class SINK>
+DACH_HD void scan_leftmost(const ScanParams& P, const RecView& V, TextWin& T, SINK& E, uint32_t len) {
     uint32_t self_pos = 0;
     uint32_t init_opos = P.root_opos;
     bool skip_empty = false;
@@ -479,6 +551,9 @@ DACH_HD void scan_leftmost(const ScanParams& P, const RecView& V, TextWin& T, Em
     DACH_WD_DECL(wd_outer);
     DACH_WD_DECL(wd_inner);
     for (;;) {
+        if constexpr (SINK::KIND == RK_FIRST) {
+            if (E.stopped()) return;
+        }
         uint32_t s = D_ROOT;
         uint4 r = root_rec;
         uint32_t last = init_opos;
@@ -1958,6 +2033,65 @@ struct StdMachine3 {
             Ev.q[0] = e;
             L.qn = 1;
         }
+    }
+};
+
+// =============================================================================================
+// COUNT and FIRST on the lane machines (StdMachine3, LmMachine, CwMachine).
+//
+// The machines queue one (end, slot) entry per output event and stop stepping when the queue is full;
+// their drain() turns entries into matches.  SinkOps<M, MODE, RK> replaces drain() and begin_item() for
+// the other two result kinds and leaves step() -- the lock-step loop -- exactly as it is:
+//   COUNT  adds 1 per event (find / no_suffix / leftmost: the head of the list) or the list's chain
+//          word (find_overlapping), without walking the list;
+//   FIRST  gives the lane a queue of depth one: begin_item() starts the queue at its last entry, so the
+//          first event fills it and the machine stops by its own rule.  If the event is reportable (it
+//          ends inside the item's segment; warm-up events do not count) its list head is the item's
+//          answer and the item is done; otherwise the queue is emptied and the lane goes on.
+// MODE is the machine's iterator: FIRST of a Standard automaton always runs the find_overlapping
+// machine, whose first event is the first event of all three Standard iterators.
+// =============================================================================================
+template <class M, int MODE, int RK>
+struct SinkOps {
+    using Sink = typename std::conditional<RK == RK_COUNT, CountSink, FirstSink>::type;
+
+    template <class LANE>
+    static DACH_HD void begin_item(LANE& L, const ScanParams& P, const StdEnv& Ev, Sink& E, uint64_t item, const uint8_t* emu_lo) {
+        Emitter unused;  // the machines only name the item to their sink
+        M::begin_item(L, P, Ev, unused, item, emu_lo);
+        E.begin((uint32_t)item);
+        if constexpr (RK == RK_FIRST) {
+            if (L.qn) {  // ROOT's list at position 0 (an empty pattern): reportable at once
+                E.emit(P, 0, 0, ld_u4(P.outputs + (ld_u32(Ev.opos + Ev.q[0].opos) - 1)).x);
+                L.qn = 0;
+                L.fl |= F_DONE | M::IDLE;
+            } else {
+                L.qn = (uint32_t)LANE_Q - 1;
+            }
+        }
+    }
+
+    template <class LANE>
+    static DACH_HD void drain(LANE& L, const StdEnv& Ev, const ScanParams& P, Sink& E) {
+        if constexpr (RK == RK_COUNT) {
+            for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j) {
+                if (j < L.qn) {
+                    const QEntry e = Ev.q[j * Ev.q_stride];
+                    if (e.end >= L.from) E.count += MODE == M_OVERLAPPING ? chain_len(P, ld_u32(Ev.opos + e.opos)) : 1u;
+                }
+            }
+            L.qn = 0;
+        } else {
+            if (L.qn == (uint32_t)LANE_Q) {
+                const QEntry e = Ev.q[(LANE_Q - 1) * Ev.q_stride];
+                if (e.end >= L.from) {
+                    emit_head(P, E, ld_u32(Ev.opos + e.opos), e.end);
+                    L.fl |= F_DONE | M::IDLE;
+                }
+            }
+            if (!(L.fl & F_DONE)) L.qn = (uint32_t)LANE_Q - 1;
+        }
+        if (!(L.fl & F_DONE)) L.fl &= ~M::IDLE;
     }
 };
 

@@ -175,6 +175,34 @@ int dach_dev_scan_stream(dach_dev *dev, int mode, const uint8_t *d_text, const u
                          dach_match *d_out, uint64_t out_cap, uint64_t *d_out_offs,
                          uint64_t *needed, void *stream);
 
+/* ---- counts and first matches ----------------------------------------------------------------
+ *
+ * Two questions that need no match list.  Same batch layout, modes, d_offs checks and errors as
+ * dach_dev_scan_batch (DACH_INVALID_ARGUMENT for bad offsets, DACH_MATCH_KIND_MISMATCH, DACH_CUDA_ERROR
+ * without a device), but no capacity: there is no DACH_OUTPUT_OVERFLOW.  The calls synchronise `stream`.
+ *
+ *   count  d_counts[i] (u64) = the number of matches iterator `mode` yields on haystack i, i.e. exactly
+ *          out_offs[i+1] - out_offs[i] of dach_dev_scan_batch; *total = their sum.  u64 because
+ *          overlapping lists make more than 2^32 matches on one haystack reachable.
+ *   first  d_first[i] = the first match iterator `mode` yields on haystack i (`iter.next()`), d_found[i] = 1
+ *          if there is one; otherwise d_found[i] = 0 and d_first[i] = {0xffffffff x 3}.  *n_found = the
+ *          haystacks with a match.  The scan of a haystack stops at its first match.  For Standard automata
+ *          the three Standard modes have the same first match (the head of the first output list reached,
+ *          ROOT's empty pattern at position 0 included).
+ *
+ * The host forms copy text and offsets to the device in the slices of dach_scan_batch_host; only the
+ * per-haystack results come back (8 B, or 13 B, per haystack; dach_dev_last_h2d_bytes / _d2h_bytes).
+ * Option kernel = 1, 2 or 4 runs the default lane machines here (kernel = 3); kernel = 0 the lane-per-haystack
+ * kernels.  Stream chunks, jobs and shard groups have no count / first form. */
+int dach_dev_count_batch(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                         uint64_t text_bytes, uint64_t *d_counts, uint64_t *total, void *stream);
+int dach_count_batch_host(dach_dev *dev, int mode, const uint8_t *text, const uint64_t *offs, uint64_t n,
+                          uint64_t *counts, uint64_t *total);
+int dach_dev_first_batch(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                         uint64_t text_bytes, dach_match *d_first, uint8_t *d_found, uint64_t *n_found, void *stream);
+int dach_first_batch_host(dach_dev *dev, int mode, const uint8_t *text, const uint64_t *offs, uint64_t n,
+                          dach_match *first, uint8_t *found, uint64_t *n_found);
+
 /* ---- asynchronous scans (jobs) ----------------------------------------------------------
  *
  * dach_dev_scan_batch is one call that synchronises its stream and serialises per handle.  A job is

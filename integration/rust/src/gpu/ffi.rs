@@ -62,6 +62,18 @@ extern "C" {
     /// Host buffers in, host buffers out.
     pub fn dach_scan_batch_host(dev: *mut DachDev, mode: i32, text: *const u8, offs: *const u64, n: u64,
                                 out: *mut DachMatch, out_cap: u64, out_offs: *mut u64, needed: *mut u64) -> i32;
+    /// Matches per haystack (u64) of iterator `mode`, no match list; *total = their sum.
+    pub fn dach_count_batch_host(dev: *mut DachDev, mode: i32, text: *const u8, offs: *const u64, n: u64,
+                                 counts: *mut u64, total: *mut u64) -> i32;
+    pub fn dach_dev_count_batch(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                                text_bytes: u64, d_counts: *mut u64, total: *mut u64, stream: *mut c_void) -> i32;
+    /// First match of iterator `mode` per haystack (`iter.next()`); found[i] = 0 and first[i] = all-ones where
+    /// there is none; *n_found = haystacks with a match.
+    pub fn dach_first_batch_host(dev: *mut DachDev, mode: i32, text: *const u8, offs: *const u64, n: u64,
+                                 first: *mut DachMatch, found: *mut u8, n_found: *mut u64) -> i32;
+    pub fn dach_dev_first_batch(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                                text_bytes: u64, d_first: *mut DachMatch, d_found: *mut u8, n_found: *mut u64,
+                                stream: *mut c_void) -> i32;
     /// Device-resident buffers.
     pub fn dach_dev_scan_batch(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
                                text_bytes: u64, d_out: *mut DachMatch, out_cap: u64, d_out_offs: *mut u64,

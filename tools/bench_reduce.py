@@ -1,0 +1,242 @@
+#!/usr/bin/env python3
+"""tools/bench_reduce.py -- counts and first matches on the bench.py workloads, one H100:
+
+    python tools/bench_reduce.py --output counts [--config C3|C3-find|C2|C4|C5] [--steps K] [--warmup W]
+    python tools/bench_reduce.py --output first  ...
+
+One step = one dach_dev_count_batch / dach_dev_first_batch on the step's batch (the batches, automata and seeds of
+bench.py).  One JSON line, bench.py's fields where they apply:
+  value              bytes offered / device time of the call's pipeline (CUDA events inside the library)
+  roofline           bench.py's definition, on the COUNT / FIRST scan kernel
+  e2e                the same batch through dach_count_batch_host / dach_first_batch_host from pinned host text
+  parity             per-haystack counts and their total (counts), or first tuples and found flags (first), against
+                     the oracle on the first --parity-frac of the last batch; and the whole step against the full
+                     matches scan of the same batch
+  first_end_frac     (first) mean first.end / haystack length over the haystacks with a match: how much of what it
+                     is offered FIRST reads
+  launches_per_step  kernels launched per step
+Nothing is written to the tree.
+"""
+import argparse
+import json
+import os
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (ROOT, os.path.join(ROOT, "tests")):
+    if p not in sys.path:
+        sys.path.insert(0, p)
+
+import numpy as np  # noqa: E402
+
+from bench import CONFIGS, UNIT, ClockSampler, Workload, measured_peaks, metric_name, mode_ids  # noqa: E402
+
+
+def reduce_parity(output, got_counts, got_first, got_found, ref_counts, ref_first, ref_found):
+    """In-run parity of --output counts / first on the oracle sample: per-haystack counts (and their total), or first
+    tuples and found flags.  got_* / ref_*: numpy arrays over the same haystacks; the first tuples may cover a prefix."""
+    if output == "counts":
+        return {"counts_equal": bool(np.array_equal(got_counts.astype(np.uint64), ref_counts.astype(np.uint64))),
+                "total_equal": int(got_counts.astype(np.uint64).sum()) == int(ref_counts.astype(np.uint64).sum())}
+    k = len(ref_first)
+    return {"found_equal": bool(np.array_equal(got_found.astype(bool), ref_found.astype(bool))),
+            "first_equal": got_first[:k].astype(np.uint32).tobytes() == ref_first.astype(np.uint32).tobytes()}
+
+
+def first_from_matches(matches, counts):
+    """(first tuples (k, 3) u32, found (k,)) of haystacks whose runs of `matches` have lengths `counts`; all-ones
+    where a haystack has none."""
+    counts = np.asarray(counts, dtype=np.int64)
+    m = np.asarray(matches).reshape(-1, 3) if not hasattr(matches, "dtype") or matches.dtype.names is None else \
+        np.stack([matches["start"], matches["end"], matches["value"]], axis=1)
+    first = np.full((len(counts), 3), 0xFFFFFFFF, dtype=np.uint32)
+    found = counts > 0
+    starts = np.concatenate([[0], np.cumsum(counts)])[:-1]
+    first[found] = m[starts[found]].astype(np.uint32)
+    return first, found
+
+
+def first_end_frac(first, found, hay_lens):
+    """mean of first.end / haystack length over the haystacks with a match (None if there is none): the share of a
+    haystack FIRST had to read."""
+    found = np.asarray(found, dtype=bool)
+    if not found.any():
+        return None
+    ends = np.asarray(first, dtype=np.uint32).reshape(-1, 3)[found, 1].astype(np.float64)
+    lens = np.asarray(hay_lens, dtype=np.float64)[found]
+    return float(np.mean(ends / np.maximum(lens, 1)))
+
+
+def run_reduce_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, t_setup):
+    """--output counts / first on one GPU: every step is one dach_dev_count_batch / dach_dev_first_batch on the step's
+    batch.  value = bytes offered / device time of the call's pipeline (CUDA events inside the library)."""
+    import torch
+
+    setup_s = time.time() - t_setup
+    counts_t = torch.empty(n, dtype=torch.int64, device=dev)
+    first_t = torch.empty((n, 3), dtype=torch.int32, device=dev)
+    found_t = torch.empty(n, dtype=torch.bool, device=dev)
+
+    def step(s):
+        t, o = batches[s % len(batches)]
+        if args.output == "counts":
+            pma.count_batch_device(dmode, t, o, out=counts_t)
+        else:
+            pma.first_batch_device(dmode, t, o, out=first_t, found=found_t)
+        st = pma.stats()
+        return st["scan_kernel_ms"], st["total_ms"]
+
+    for s in range(args.warmup):
+        step(s)
+    torch.cuda.synchronize()
+    sampler = ClockSampler(dev.index)
+    sampler.start()
+    time.sleep(0.2)
+    n_before = len(sampler.rows)
+    launches1 = pma.stats()["launches"]
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    times = [step(args.warmup + s) for s in range(args.steps)]
+    ev1.record()
+    torch.cuda.synchronize()
+    time.sleep(0.25)
+    clocks = sampler.stop(skip=n_before)
+    launches2 = pma.stats()["launches"]
+    wall_ms = ev0.elapsed_time(ev1) / args.steps
+    k_ms = float(np.mean([t[0] for t in times]))
+    dev_ms = float(np.mean([t[1] for t in times]))
+    value = step_bytes / (dev_ms * 1e-3) / 1e9
+    last_batch = (args.warmup + args.steps - 1) % len(batches)
+    t_last, o_last = batches[last_batch]
+    # the full scan of the same batch (untimed): its per-haystack runs are what counts / first must equal
+    r = pma.scan_batch_device(dmode, t_last, o_last)
+    full_counts = torch.diff(r.offsets)
+    extra = {}
+    if args.output == "counts":
+        step_ok = bool(torch.equal(counts_t, full_counts))
+        extra["total"] = int(counts_t.sum().item())
+    else:
+        fd = full_counts > 0
+        step_ok = bool(torch.equal(found_t, fd)) and bool(torch.equal(first_t[fd], r.matches[r.offsets[:-1][fd]]))
+        extra["n_found"] = int(found_t.sum().item())
+        hl = torch.diff(o_last).cpu().numpy()
+        extra["first_end_frac"] = first_end_frac(first_t.cpu().numpy().view(np.uint32), found_t.cpu().numpy(), hl)
+    del r, full_counts
+    parity = None
+    if not args.no_cpu:
+        import oracle_api as O
+
+        threads = O.cpu_budget()["threads"]
+        ns = max(1, min(n, int(n * args.parity_frac)))
+        nt = max(1, ns // 4)
+        opma = W.oracle()
+        lo = W.batch_ranges()[last_batch][0]
+        ptext, poffs = W.host_batch(lo, lo + ns)
+        ref = opma.scan_batch(omode, ptext, poffs, nthreads=threads, want_hashes=False)
+        ref_t = opma.scan_batch(omode, ptext[: int(poffs[nt])], poffs[: nt + 1], nthreads=threads, want_matches=True)
+        ref_first, _ = first_from_matches(ref_t["matches"], ref_t["counts"])
+        parity = reduce_parity(args.output, counts_t[:ns].cpu().numpy(), first_t[:ns].cpu().numpy().view(np.uint32),
+                               found_t[:ns].cpu().numpy(), ref["counts"], ref_first, ref["counts"] > 0)
+        parity.update({"haystacks_checked": ns, "share_of_batch": ns / n, "first_tuples_checked": nt if args.output == "first" else 0,
+                       "what": "last timed step vs the oracle on the first %d haystacks of its batch" % ns})
+    parity = dict(parity or {}, step_equals_full_scan=step_ok)
+    e2e = None
+    if not args.no_e2e:
+        t0_, o0_ = batches[0]
+        h_text_t = torch.empty(t0_.numel(), dtype=torch.uint8).pin_memory()  # as the matches path: pinned host text
+        h_text_t.copy_(t0_)
+        h_text = h_text_t.numpy()
+        h_offs = o0_.cpu().numpy().astype(np.uint64)
+        e2e_ms = []
+        for i in range(1 + args.e2e_steps):
+            t0 = time.perf_counter()
+            if args.output == "counts":
+                pma.count_batch_host(dmode, h_text, h_offs)
+            else:
+                pma.first_batch_host(dmode, h_text, h_offs)
+            if i >= 1:
+                e2e_ms.append((time.perf_counter() - t0) * 1e3)
+        st = pma.stats()
+        e2e = {"value": h_text.size / (np.mean(e2e_ms) * 1e-3) / 1e9, "unit": UNIT, "h2d_bytes_per_step": int(st["h2d_bytes"]),
+               "d2h_bytes_per_step": int(st["d2h_bytes"]), "ms_per_step": float(np.mean(e2e_ms)),
+               "workload": "the step batch's %d haystacks x %d B through the host entry point: pinned host text -> device -> "
+                           "scan -> per-haystack results to pageable host arrays" % (n, hay_len)}
+        del h_text_t
+    peak, peak_src = measured_peaks()
+    achieved = step_bytes / (k_ms * 1e-3) / 1e9
+    roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
+                "kernel": "k_scan_machine_rk (%s)" % args.output, "kernel_ms": k_ms, "algorithmic_bytes_per_launch": step_bytes,
+                "peak_source": peak_src,
+                "note": "algorithmic bytes = 1 B read per haystack byte offered; kernel_ms = mean CUDA-event time of the scan kernel"}
+    return {
+        "metric": metric_name(W.spec) + ", " + args.output, "output": args.output, "value": value, "unit": UNIT, "n_gpus": 1,
+        "steps": args.steps, "warmup": args.warmup, "ms_per_step": wall_ms, "device_ms_per_step": dev_ms, "higher_is_better": True,
+        "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
+        "config": {"workload": "%s: %s, %s, %d haystacks x %d B per step, %d batch(es) resident (%.2f GiB)" % (
+                       args.config, W.spec["what"], W.mode_name, n, hay_len, len(batches), resident / 2**30),
+                   "n_patterns": len(W.ps), "hay_len": hay_len, "bytes_per_gpu": step_bytes, "options": args.option,
+                   "setup_s": setup_s},
+        **extra, "roofline": roofline, "parity": parity, "e2e": e2e,
+        "gpu_launches": int(launches2 - launches1), "launches_per_step": (launches2 - launches1) / args.steps, "clocks": clocks,
+    }
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--output", required=True, choices=["counts", "first"])
+    ap.add_argument("--config", default="C3", choices=sorted(CONFIGS))
+    ap.add_argument("--steps", type=int, default=None)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--scale", type=float, default=1.0, help="fraction of the config's batch (debug only)")
+    ap.add_argument("--pool-mib", type=int, default=None)
+    ap.add_argument("--e2e-steps", type=int, default=3)
+    ap.add_argument("--parity-frac", type=float, default=0.04, help="share of a batch checked against the oracle")
+    ap.add_argument("--option", action="append", default=[], help="kernel option name=value")
+    ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--no-cpu", action="store_true", help="no oracle parity")
+    args = ap.parse_args()
+    if args.steps is None:
+        args.steps = CONFIGS[args.config]["steps"]
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+
+    import torch
+
+    from daachorse_b200 import synth as S
+
+    assert torch.cuda.is_available(), "bench_reduce.py needs a CUDA device (no CPU fallback)"
+    torch.cuda.set_device(0)
+    dev = torch.device("cuda", 0)
+    t_setup = time.time()
+    W = Workload(args.config, args.scale, 0, args.pool_mib)
+    dmode, omode = mode_ids(W.mode_name)
+    hay_len = W.hay_len
+    pma = W.automaton()
+    for kv in args.option:
+        k, v = kv.split("=")
+        pma.set_option(k, int(v))
+    pool_t = torch.from_numpy(W.pool).to(dev)
+    starts_t = torch.from_numpy(W.starts).to(dev)
+    ranges = W.batch_ranges()
+    if "window" in W.spec:
+        text_all, offs_all = S.materialise_on_device(pool_t, starts_t, hay_len)
+        batches = [(text_all[lo * hay_len: hi * hay_len], offs_all[: hi - lo + 1]) for lo, hi in ranges]
+        resident = text_all.numel()
+    else:
+        batches = []
+        for lo, hi in ranges:
+            t, o = S.materialise_on_device(pool_t, starts_t[lo:hi], hay_len)
+            if W.spec["synth"] == "C4":
+                S.pad_to_char_boundary_device(t, hi - lo, hay_len)
+            batches.append((t, o))
+        resident = sum(b[0].numel() for b in batches)
+    del pool_t
+    n = W.window
+    torch.cuda.synchronize()
+    line = run_reduce_output(args, W, pma, batches, dmode, omode, n, hay_len, n * hay_len, resident, dev, t_setup)
+    print(json.dumps(line), flush=True)
+
+
+if __name__ == "__main__":
+    main()

@@ -7,7 +7,7 @@ native, so this is a subset of tests/test_gpu_parity.py that still launches ever
 
 Golden vectors (all iterators x bytewise / charwise), random batches on every kernel option, text buffers at odd
 addresses and with no slack after the last byte (the 8-byte text loads must not touch anything outside), stream
-chunks, asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
+chunks, counts and first matches, asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
 import json
 import os
 import sys
@@ -89,6 +89,39 @@ def random_batches():
                 n_scans += 1
 
 
+def counts_and_first():
+    """dach_count_batch_host / dach_first_batch_host on every kernel that serves them, the device forms on text at an
+    odd address; against the oracle's per-haystack runs."""
+    global n_scans
+    dev = torch.device("cuda", 0)
+    for cw in (False, True):
+        for kind in (0, 1):
+            pma, opma, text, offs = random_case(20 + 10 * kind + cw, cw, kind)
+            for mode in ([D.LEFTMOST_FIND] if kind else [D.FIND, D.FIND_OVERLAPPING, D.FIND_OVERLAPPING_NO_SUFFIX]):
+                ref = opma.scan_batch(ORC[mode], text, offs, want_matches=True)
+                counts = ref["counts"].astype(np.uint64)
+                starts = np.concatenate([[0], np.cumsum(counts)])[:-1].astype(np.int64)
+                found = counts > 0
+                for opts in ({"kernel": 3}, {"kernel": 3, "hot_entries": 512}, {"kernel": 0}, {"kernel": 3, "seg_len": 64}):
+                    for k, v in opts.items():
+                        pma.set_option(k, v)
+                    c, _ = pma.count_batch_host(mode, text, offs)
+                    f, fd = pma.first_batch_host(mode, text, offs)
+                    assert np.array_equal(c, counts) and np.array_equal(fd, found), (cw, kind, mode, opts)
+                    assert f[fd].tobytes() == ref["matches"][starts[found]].tobytes(), (cw, kind, mode, opts)
+                    n_scans += 2
+                    pma.set_option("seg_len", 0)
+                    pma.set_option("hot_entries", 0)
+                pma.set_option("kernel", 3)
+                pad = 3
+                buf = torch.empty(text.size + pad, dtype=torch.uint8, device=dev)
+                buf[pad:] = torch.from_numpy(text.copy()).to(dev)
+                o = torch.from_numpy(offs.astype(np.int64)).to(dev)
+                assert np.array_equal(pma.count_batch_device(mode, buf[pad:], o).cpu().numpy().astype(np.uint64), counts)
+                assert np.array_equal(pma.first_batch_device(mode, buf[pad:], o)[1].cpu().numpy(), found)
+                n_scans += 2
+
+
 def streams_jobs_groups():
     global n_scans
     dev = torch.device("cuda", 0)
@@ -148,6 +181,7 @@ def streams_jobs_groups():
 if __name__ == "__main__":
     golden()
     random_batches()
+    counts_and_first()
     streams_jobs_groups()
     torch.cuda.synchronize()
     print("sanitize.py: %d scans, all equal to the oracle" % n_scans)
