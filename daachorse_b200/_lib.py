@@ -16,10 +16,11 @@ LIB_PATH = os.environ.get("DACH_LIB") or os.path.join(_DIR, "libdaachorse_b200.s
 SYMBOLS = [
     "dach_bytewise_build", "dach_charwise_build", "dach_pma_deserialize", "dach_pma_serialized_bytes",
     "dach_pma_serialize", "dach_pma_match_kind", "dach_pma_num_states", "dach_pma_heap_bytes",
-    "dach_pma_num_elements", "dach_pma_is_charwise", "dach_pma_max_pattern_len", "dach_pma_free",
+    "dach_pma_num_elements", "dach_pma_is_charwise", "dach_pma_max_pattern_len", "dach_pma_num_outputs",
+    "dach_pma_outputs", "dach_pma_free",
     "dach_dev_upload", "dach_dev_free", "dach_dev_image_bytes", "dach_dev_scan_batch", "dach_dev_scan_stream",
     "dach_scan_batch_host", "dach_dev_count_batch", "dach_count_batch_host", "dach_dev_first_batch", "dach_first_batch_host",
-    "dach_dev_kernel_launches", "dach_dev_last_scan_kernel_ms",
+    "dach_dev_hist_batch", "dach_hist_batch_host", "dach_dev_kernel_launches", "dach_dev_last_scan_kernel_ms",
     "dach_dev_last_total_ms", "dach_dev_last_h2d_bytes", "dach_dev_last_d2h_bytes",
     "dach_dev_set_option", "dach_last_error", "dach_abi_version",
     "dach_job_create", "dach_job_free", "dach_job_scan", "dach_job_place", "dach_job_wait", "dach_job_scan_kernel_ms", "dach_job_push_ms", "dach_job_times",
@@ -55,9 +56,12 @@ def load():
     L.dach_pma_serialize.restype = C.c_int
     for name, rt in (("dach_pma_match_kind", C.c_uint8), ("dach_pma_num_states", C.c_uint32),
                      ("dach_pma_heap_bytes", C.c_size_t), ("dach_pma_num_elements", C.c_size_t),
-                     ("dach_pma_is_charwise", C.c_int), ("dach_pma_max_pattern_len", C.c_uint32)):
+                     ("dach_pma_is_charwise", C.c_int), ("dach_pma_max_pattern_len", C.c_uint32),
+                     ("dach_pma_num_outputs", C.c_uint32)):
         getattr(L, name).argtypes = [vp]
         getattr(L, name).restype = rt
+    L.dach_pma_outputs.argtypes = [vp, vp, vp, vp, C.c_uint32]
+    L.dach_pma_outputs.restype = C.c_int
     L.dach_pma_free.argtypes = [vp]
     L.dach_pma_free.restype = None
     L.dach_dev_upload.argtypes = [vp, C.c_int, pp]
@@ -79,7 +83,10 @@ def load():
     L.dach_count_batch_host.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, vp, C.POINTER(C.c_uint64)]
     L.dach_dev_first_batch.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, C.c_uint64, vp, vp, C.POINTER(C.c_uint64), vp]
     L.dach_first_batch_host.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, vp, vp, C.POINTER(C.c_uint64)]
-    for name in ("dach_dev_count_batch", "dach_count_batch_host", "dach_dev_first_batch", "dach_first_batch_host"):
+    L.dach_dev_hist_batch.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_uint64, C.c_uint64, vp, C.c_uint64, C.POINTER(C.c_uint64), vp]
+    L.dach_hist_batch_host.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_uint64, vp, C.c_uint64, C.POINTER(C.c_uint64)]
+    for name in ("dach_dev_count_batch", "dach_count_batch_host", "dach_dev_first_batch", "dach_first_batch_host",
+                 "dach_dev_hist_batch", "dach_hist_batch_host"):
         getattr(L, name).restype = C.c_int
     L.dach_dev_kernel_launches.argtypes = [vp]
     L.dach_dev_kernel_launches.restype = C.c_uint64

@@ -31,6 +31,7 @@ from . import _lib
 MATCH_DTYPE = np.dtype([("start", "<u4"), ("end", "<u4"), ("value", "<u4")])
 
 FIND, FIND_OVERLAPPING, FIND_OVERLAPPING_NO_SUFFIX, LEFTMOST_FIND = range(4)
+HIST_KEYS = {"output": 0, "value": 1}  # dach_hist_key
 
 
 class MatchKind(enum.IntEnum):
@@ -208,6 +209,24 @@ class _Automaton:
 
     def max_pattern_len(self):
         return _lib.load().dach_pma_max_pattern_len(self._h)
+
+    def outputs(self):
+        """The output records as numpy uint32 arrays ``(values, lengths, parents)``: one record per pattern the builder
+        kept (duplicates get one each); parent 0 = none, else the parent's 1-based index.  Index i labels bin i of a
+        ``key="output"`` histogram."""
+        L = _lib.load()
+        k = int(L.dach_pma_num_outputs(self._h))
+        vals, lens, pars = (np.zeros(max(k, 1), dtype=np.uint32) for _ in range(3))
+        _check(L.dach_pma_outputs(self._h, _ptr(vals), _ptr(lens), _ptr(pars), k))
+        return vals[:k], lens[:k], pars[:k]
+
+    def _hist_len(self, key):
+        if key not in HIST_KEYS:
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "key must be 'value' or 'output'")
+        vals = self.outputs()[0]
+        if key == "output":
+            return len(vals)
+        return int(vals.max()) + 1 if len(vals) else 0
 
     def serialize(self):
         L = _lib.load()
@@ -424,6 +443,49 @@ class _Automaton:
                                                 C.c_void_p(out.data_ptr()), C.c_void_p(found.data_ptr()), C.byref(nf), st))
         return out, found
 
+    def pattern_counts_host(self, mode, text, offs, key="value", out=None, device=None):
+        """How often each pattern occurs in the batch, host buffers in and out: ``np.uint64`` histogram, added into
+        ``out`` if given (zeros otherwise).  ``key="value"``: bin = the match's value (a bincount of the values of
+        ``scan_batch_host``); ``key="output"``: bin = the match's output record (``outputs()``).  No match list."""
+        text, offs, n = self._host_batch_args(mode, text, offs)
+        L = _lib.load()
+        d = self.device_handle(device)
+        need = self._hist_len(key)
+        if out is None:
+            out = np.zeros(need, dtype=np.uint64)
+        elif out.dtype != np.uint64 or out.ndim != 1 or not out.flags.c_contiguous or not out.flags.writeable:
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "out must be a writable contiguous 1-d uint64 array")
+        total = C.c_uint64()
+        _check(L.dach_hist_batch_host(d, mode, HIST_KEYS[key], _ptr(text), C.c_void_p(offs.ctypes.data), n, _ptr(out), out.size,
+                                      C.byref(total)))
+        return out
+
+    def pattern_counts_device(self, mode, text, offs, key="value", out=None, stream=None):
+        """Device-resident form of ``pattern_counts_host``: ``text`` / ``offs`` as in ``scan_batch_device``; returns the
+        int64 CUDA histogram, added into ``out`` if given (zeros otherwise) -- calls on consecutive batches accumulate
+        a corpus on the device."""
+        import torch
+
+        self._assert_mode(mode)
+        dev = text.device.index if text.device.index is not None else torch.cuda.current_device()
+        need = self._hist_len(key)
+        if out is None:
+            out = torch.zeros(need, dtype=torch.int64, device=text.device)
+        _check_device_batch(text, offs, dev, hist=out, hist_len=need)
+        d = self.device_handle(dev)
+        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
+        total = C.c_uint64()
+        _check(_lib.load().dach_dev_hist_batch(d, mode, HIST_KEYS[key], C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()),
+                                               offs.numel() - 1, text.numel(), C.c_void_p(out.data_ptr()), out.numel(),
+                                               C.byref(total), st))
+        return out
+
+    def value_counts_batch(self, haystacks, mode=None):
+        """Occurrences per value over all haystacks: ``np.uint64[max value + 1]`` (for ``new`` automata: per pattern);
+        ``mode=None`` as in ``count_batch``."""
+        blob, offs = _pack(list(haystacks), self._charwise)
+        return self.pattern_counts_host(self._default_mode(mode), blob, offs, key="value")
+
     def _default_mode(self, mode):
         if mode is not None:
             return mode
@@ -560,7 +622,7 @@ def torch_int64():
 
 
 def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=None, pos=None, counts=None, first=None,
-                        found=None):
+                        found=None, hist=None, hist_len=0):
     """Raw pointers cross the C ABI: a wrong dtype, stride or device would be silent garbage or a device fault."""
     import torch
 
@@ -574,7 +636,7 @@ def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=No
                             ("out", out, (torch.int32, torch.uint32)), ("out_offs", out_offs, (torch.int64, torch.uint64)),
                             ("state", state, (torch.int32, torch.uint32)), ("pos", pos, (torch.int32, torch.uint32)),
                             ("counts", counts, (torch.int64, torch.uint64)), ("first", first, (torch.int32, torch.uint32)),
-                            ("found", found, (torch.bool, torch.uint8))):
+                            ("found", found, (torch.bool, torch.uint8)), ("hist", hist, (torch.int64,))):
         if t is None:
             continue
         if not t.is_cuda or t.device.index != dev_index:
@@ -592,6 +654,8 @@ def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=No
             bad("%s must hold n entries" % name)
     if first is not None and (first.dim() != 2 or first.shape[0] != n or first.shape[1] != 3):
         bad("first must have shape (n, 3)")
+    if hist is not None and (hist.dim() != 1 or hist.numel() < hist_len):
+        bad("hist must be 1-d with at least %d entries" % hist_len)
 
 
 def _current_device():

@@ -88,6 +88,21 @@ uint32_t dach_pma_max_pattern_len(const dach_pma* pma) {
     return m;
 }
 
+uint32_t dach_pma_num_outputs(const dach_pma* pma) { return pma ? (uint32_t)pma->outputs.size() : 0; }
+
+int dach_pma_outputs(const dach_pma* pma, uint32_t* values, uint32_t* lengths, uint32_t* parents, uint32_t n) {
+    if (!pma || n < pma->outputs.size()) {
+        set_error("dach_pma_outputs: null automaton or n below the number of output records");
+        return DACH_INVALID_ARGUMENT;
+    }
+    for (size_t i = 0; i < pma->outputs.size(); ++i) {
+        if (values) values[i] = pma->outputs[i].value;
+        if (lengths) lengths[i] = pma->outputs[i].length;
+        if (parents) parents[i] = pma->outputs[i].parent;
+    }
+    return DACH_OK;
+}
+
 void dach_pma_free(dach_pma* pma) { delete pma; }
 
 }  // extern "C"

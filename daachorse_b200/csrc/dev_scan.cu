@@ -12,8 +12,9 @@
 //       k_scan_duo<MODE>        StdMachine3 with two haystacks per lane (option kernel = 4; measured slower)
 //       k_scan<CHARWISE, MODE>  lane per haystack, reference-shaped loop: automata above 2^24 slots, find_iter with
 //                               an empty pattern, and option kernel = 0
-//     k_scan_machine_rk / k_scan_rk  the same machines / loops with a COUNT or FIRST sink (dach_dev_count_batch,
-//                               dach_dev_first_batch), followed by k_count_hay / k_first_hay (per-haystack results)
+//     k_scan_machine_rk / k_scan_rk  the same machines / loops with a COUNT, FIRST or HIST sink (dach_dev_count_batch,
+//                               dach_dev_first_batch, dach_dev_hist_batch), followed by k_count_hay / k_first_hay
+//                               (per-haystack results) or k_hist_heads / k_hist_fold (per-pattern counts)
 //     k_offsets_*               exclusive scan of the per-item match counts
 //     k_blk_index               pool blocks listed in output order (large batches)
 //   phase 2
@@ -58,7 +59,9 @@ constexpr uint32_t kRootBytes = 1024;  // 256 x u32 at the front of dynamic shar
 
 // the result sink of each result kind
 template <int RK>
-using SinkOf = typename std::conditional<RK == RK_COUNT, CountSink, typename std::conditional<RK == RK_FIRST, FirstSink, Emitter>::type>::type;
+using SinkOf = typename std::conditional<
+    RK == RK_COUNT, CountSink,
+    typename std::conditional<RK == RK_FIRST, FirstSink, typename std::conditional<RK == RK_HIST, HistSink, Emitter>::type>::type>::type;
 
 template <bool CHARWISE, int MODE, class SINK>
 __device__ __forceinline__ void scan_items(const ScanParams& P) {
@@ -166,6 +169,13 @@ __device__ __forceinline__ void scan_machine(const ScanParams& P) {
     L.qn = 0;
     SINK E;
     E.begin(0);
+    if constexpr (SINK::KIND == RK_HIST) {
+        // HIST: u32 counters of compact slots [0, hist_smem) behind the queues
+        E.s_cnt = reinterpret_cast<unsigned int*>(s_queue + (size_t)LANE_Q * blockDim.x);
+        E.k = P.hist_smem;
+        for (uint32_t i = threadIdx.x; i < P.hist_smem; i += blockDim.x) E.s_cnt[i] = 0;
+        __syncthreads();
+    }
     bool exhausted = false;
     const unsigned long long n_items = P.n_items_dev ? *P.n_items_dev : P.n_items;
     if (HOT) mbar_wait(&s_bar, 0);
@@ -222,6 +232,11 @@ __device__ __forceinline__ void scan_machine(const ScanParams& P) {
                 }
             }
         }
+    }
+    if constexpr (SINK::KIND == RK_HIST) {  // the CTA's shared-memory counts, once
+        __syncthreads();
+        for (uint32_t i = threadIdx.x; i < P.hist_smem; i += blockDim.x)
+            if (E.s_cnt[i]) red_add_u64(P.slot_hist + i, E.s_cnt[i]);
     }
 }
 
@@ -730,6 +745,38 @@ __global__ void __launch_bounds__(256) k_first_hay(const unsigned long long* seg
     add_block_total(v, n_found);
 }
 
+// ---- HIST: per-record counts from per-slot counts, then the caller's keys -------------------------------------------
+// k_hist_heads   (lane machines) slot s counted events of its state: they go to the record that heads the state's
+//                list (opos[s]).  Several slots may share a head.
+// k_hist_fold    every record i with a count v: hist[key(j)] += v for j = i, and with CHAIN (find_overlapping on the
+//                lane machines, where an event reports the whole list) for every record on i's parent chain too.
+//                key(j) = j (output key) or value(j) (value key).  *total += the matches added.
+__global__ void __launch_bounds__(256) k_hist_heads(const unsigned long long* slot_hist, const uint32_t* opos, uint32_t n_slots,
+                                                     unsigned long long* rec_hist) {
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += gridDim.x * blockDim.x) {
+        const unsigned long long v = slot_hist[s];
+        const uint32_t op = v ? opos[s] : 0u;
+        if (op) red_add_u64(rec_hist + (op - 1), v);
+    }
+}
+
+template <bool CHAIN>
+__global__ void __launch_bounds__(256) k_hist_fold(const unsigned long long* rec_hist, const uint4* outputs, uint32_t n_out, int key_value,
+                                                    unsigned long long* hist, unsigned long long* total) {
+    unsigned long long added = 0;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_out; i += gridDim.x * blockDim.x) {
+        const unsigned long long v = rec_hist[i];
+        uint32_t j = v ? i + 1 : 0u;  // 1-based
+        while (j) {
+            const uint4 o = outputs[j - 1];
+            red_add_u64(hist + (key_value ? o.x : j - 1), v);
+            added += v;
+            j = CHAIN ? o.z : 0u;
+        }
+    }
+    add_block_total(added, total);
+}
+
 }  // namespace dach
 
 // ------------------------------------------------------------------------------------------
@@ -778,6 +825,7 @@ struct Workspace {
     DevBuf blk_first, blkmap, tiles2;  // pool blocks in output order (k_blk_index)
     DevBuf stage;  // shard groups: the job's dense matches, pushed to the gathering rank by k_push
     DevBuf items_rk, total_rk;  // COUNT / FIRST: per-item results, the batch's total (u64)
+    DevBuf slot_hist, rec_hist, hist_acc;  // HIST: per compact slot, per output record; host form: the batch's histogram
     HostPinned* pinned = nullptr;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // pipeline start, scan end, pipeline end, scan start
     cudaEvent_t ev_scanned = nullptr, ev_placed = nullptr;
@@ -808,7 +856,8 @@ struct Workspace {
     }
     void release() {
         for (DevBuf* b : {&counts, &tiles, &ctrl, &pool, &text, &offs, &out, &out_offs, &nseg, &seg_first, &item_hay, &item_beg,
-                          &item_offs, &n_items_dev, &blk_first, &blkmap, &tiles2, &stage, &items_rk, &total_rk})
+                          &item_offs, &n_items_dev, &blk_first, &blkmap, &tiles2, &stage, &items_rk, &total_rk, &slot_hist, &rec_hist,
+                          &hist_acc})
             if (b->p) {
                 cudaFree(b->p);
                 b->p = nullptr;
@@ -845,6 +894,7 @@ struct dach_dev {
     uint8_t match_kind = 0;
     uint32_t n_slots = 0, root_opos = 0, mapper_len = 0, max_pattern_len = 0;
     bool segmentable = false;  // HostImage::segmentable: long haystacks may be cut into segments
+    uint32_t n_outputs = 0, max_value = 0, n_cslots = 0;  // output records, their largest value, compact slots
     size_t image_bytes = 0;
     int sm_count = 0;
     size_t smem_optin = 0;
@@ -875,6 +925,9 @@ struct dach_dev {
     // the carveout leaves L1 too small for the misses in flight; 6144 keeps a margin.  0 = off, -1 = as many as fit
     // next to the event queues.
     int64_t opt_hot_entries = 6144;
+    // HIST on the lane machines: events of the leading compact slots are counted in shared memory per CTA (4 B
+    // each, next to the hot records and the queues) before they reach global memory.  0 = off.
+    int64_t opt_hist_smem = 1024;
     int64_t opt_slice_ramp = 1;      // host path: small slices at the head and the tail of a batch
     int64_t opt_tail_seg = 0;        // cut only the last 2 x lanes haystacks of a large batch (off by default)
     int64_t opt_gather_ordered = 1;  // copy pool blocks in output order (sequential writes)
@@ -1059,18 +1112,19 @@ cudaError_t launch_scan_rk_t(const ScanParams& P, int grid, int threads, size_t 
 }
 
 // which: 3 StdMachine3 (bytewise Standard), 1 LmMachine / CwMachine (by the automaton), 0 lane per haystack.
-// FIRST only runs M_OVERLAPPING (Standard) and M_LEFTMOST: the caller folds the Standard modes.
+// FIRST only runs M_OVERLAPPING (Standard) and M_LEFTMOST: the caller folds the Standard modes.  HIST runs all of
+// COUNT's kernels.
 template <int RK>
 cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
     if (which == 3) {
         switch (mode) {
             case M_FIND:
-                if constexpr (RK == RK_COUNT)
+                if constexpr (RK == RK_COUNT || RK == RK_HIST)
                     return P.hot_entries ? launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, RK, true>(P, grid, threads, smem, st)
                                          : launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, RK, false>(P, grid, threads, smem, st);
                 break;
             case M_NO_SUFFIX:
-                if constexpr (RK == RK_COUNT)
+                if constexpr (RK == RK_COUNT || RK == RK_HIST)
                     return P.hot_entries ? launch_rk_t<StdMachine3<M_NO_SUFFIX>, Lane3, M_NO_SUFFIX, RK, true>(P, grid, threads, smem, st)
                                          : launch_rk_t<StdMachine3<M_NO_SUFFIX>, Lane3, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
                 break;
@@ -1083,10 +1137,10 @@ cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int gri
     if (which == 1 && cw) {
         switch (mode) {
             case M_FIND:
-                if constexpr (RK == RK_COUNT) return launch_rk_t<CwMachine<M_FIND>, LaneCw, M_FIND, RK, false>(P, grid, threads, smem, st);
+                if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_rk_t<CwMachine<M_FIND>, LaneCw, M_FIND, RK, false>(P, grid, threads, smem, st);
                 break;
             case M_NO_SUFFIX:
-                if constexpr (RK == RK_COUNT) return launch_rk_t<CwMachine<M_NO_SUFFIX>, LaneCw, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
+                if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_rk_t<CwMachine<M_NO_SUFFIX>, LaneCw, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
                 break;
             case M_OVERLAPPING: return launch_rk_t<CwMachine<M_OVERLAPPING>, LaneCw, M_OVERLAPPING, RK, false>(P, grid, threads, smem, st);
             case M_LEFTMOST: return launch_rk_t<CwMachine<M_LEFTMOST>, LaneCw, M_LEFTMOST, RK, false>(P, grid, threads, smem, st);
@@ -1095,13 +1149,13 @@ cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int gri
     }
     if (which == 1) return mode == M_LEFTMOST ? launch_rk_t<LmMachine, LaneLm, M_LEFTMOST, RK, false>(P, grid, threads, smem, st) : cudaErrorInvalidValue;
     switch ((cw ? 4 : 0) + mode) {
-        case 0: if constexpr (RK == RK_COUNT) return launch_scan_rk_t<false, M_FIND, RK>(P, grid, threads, smem, st); break;
+        case 0: if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_scan_rk_t<false, M_FIND, RK>(P, grid, threads, smem, st); break;
         case 1: return launch_scan_rk_t<false, M_OVERLAPPING, RK>(P, grid, threads, smem, st);
-        case 2: if constexpr (RK == RK_COUNT) return launch_scan_rk_t<false, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
+        case 2: if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_scan_rk_t<false, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
         case 3: return launch_scan_rk_t<false, M_LEFTMOST, RK>(P, grid, threads, smem, st);
-        case 4: if constexpr (RK == RK_COUNT) return launch_scan_rk_t<true, M_FIND, RK>(P, grid, threads, smem, st); break;
+        case 4: if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_scan_rk_t<true, M_FIND, RK>(P, grid, threads, smem, st); break;
         case 5: return launch_scan_rk_t<true, M_OVERLAPPING, RK>(P, grid, threads, smem, st);
-        case 6: if constexpr (RK == RK_COUNT) return launch_scan_rk_t<true, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
+        case 6: if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_scan_rk_t<true, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
         case 7: return launch_scan_rk_t<true, M_LEFTMOST, RK>(P, grid, threads, smem, st);
     }
     return cudaErrorInvalidValue;
@@ -1158,11 +1212,13 @@ ScanParams image_params(const dach_dev* d, const uint8_t* d_text, const uint8_t*
 
 // dynamic shared memory of the scan kernel: the lane machines' event queues (queue_sets per lane) and, for
 // StdMachine3, the front of the hot region; the lane-per-haystack kernels stage leading wide records
-size_t plan_smem(const dach_dev* d, ScanParams& P, bool v1, bool std3, int threads, int ctas_per_sm, int queue_sets) {
+size_t plan_smem(const dach_dev* d, ScanParams& P, bool v1, bool std3, int threads, int ctas_per_sm, int queue_sets,
+                 uint32_t hist_smem = 0) {
     const size_t smem_budget = std::min<size_t>(d->smem_optin, 226 * 1024) / ctas_per_sm - (ctas_per_sm > 1 ? 1024 : 0);
     size_t smem;
     if (v1) {
-        const size_t queues = (size_t)LANE_Q * threads * sizeof(QEntry) * queue_sets;
+        // HIST: hist_smem u32 counters behind the queues (counted with them: they come before the hot records)
+        const size_t queues = (size_t)LANE_Q * threads * sizeof(QEntry) * queue_sets + (size_t)hist_smem * 4;
         // StdMachine3: the front of the hot region next to the queues (whole 256-slot blocks)
         uint64_t want = 0;
         if (std3 && d->opt_hot_entries != 0 && smem_budget > queues + 512) {
@@ -1671,13 +1727,14 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
     return DACH_OK;
 }
 
-// ---- COUNT / FIRST: the scan of a batch and its per-haystack results on one stream.  No synchronisation. ----------
-// rk = RK_COUNT: d_counts (n x u64); RK_FIRST: d_first (n tuples), d_found (n x u8).  The total (matches, or haystacks
-// with a match) lands in W.pinned->total_rk once W.ev_placed has completed.  No block pool, no offsets, no gather:
-// options kernel = 1, 2, 4 run StdMachine3 here (kernel = 0: the lane-per-haystack kernels).
+// ---- COUNT / FIRST / HIST: the scan of a batch and its results on one stream.  No synchronisation. ----------------
+// rk = RK_COUNT: d_counts (n x u64); RK_FIRST: d_first (n tuples), d_found (n x u8); RK_HIST: added into d_hist by
+// `key` (DACH_KEY_OUTPUT / DACH_KEY_VALUE; the caller has checked its size).  The total (matches, or haystacks with a
+// match) lands in W.pinned->total_rk once W.ev_placed has completed.  No block pool, no offsets, no gather: options
+// kernel = 1, 2, 4 run StdMachine3 here (kernel = 0: the lane-per-haystack kernels).
 int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
                uint64_t text_bytes, const uint64_t* d_offs, uint64_t n, uint64_t* d_counts, dach_match* d_first, uint8_t* d_found,
-               cudaStream_t st) {
+               cudaStream_t st, int key = 0, uint64_t* d_hist = nullptr) {
     if (n > 0xfffffff0ull) {
         set_error("too many haystacks in one batch (max 2^32-16)");
         return DACH_INVALID_ARGUMENT;
@@ -1721,7 +1778,7 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             }
         }
         const uint64_t n_tiles = (n + kScanTile - 1) / kScanTile;
-        if (!ensure(W.items_rk, n_items_max * (rk == RK_FIRST ? 16 : 8))) return DACH_CUDA_ERROR;
+        if (rk != RK_HIST && !ensure(W.items_rk, n_items_max * (rk == RK_FIRST ? 16 : 8))) return DACH_CUDA_ERROR;
         if (seg && (!ensure(W.tiles, n_tiles * 8) || !ensure(W.nseg, n * 4) || !ensure(W.seg_first, (n + 1) * 8) ||
                     !ensure(W.item_hay, n_items_max * 4) || !ensure(W.item_beg, n_items_max * 4) || !ensure(W.n_items_dev, 8)))
             return DACH_CUDA_ERROR;
@@ -1729,24 +1786,52 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         P.ctrl = static_cast<ScanCtrl*>(W.ctrl.p);
         P.item_count = static_cast<unsigned long long*>(W.items_rk.p);
         P.item_first = static_cast<uint4*>(W.items_rk.p);
-        const size_t smem = plan_smem(d, P, machine, std3, threads, ctas_per_sm, 1);
+        uint32_t hist_k = 0;
+        if (rk == RK_HIST) {
+            if (machine) hist_k = (uint32_t)std::min<int64_t>(std::max<int64_t>(d->opt_hist_smem, 0), std::min<int64_t>(d->n_cslots, 16384));
+            if ((machine && !ensure(W.slot_hist, (size_t)d->n_cslots * 8)) || !ensure(W.rec_hist, (size_t)d->n_outputs * 8))
+                return DACH_CUDA_ERROR;
+            if ((machine && !cuda_ok(cudaMemsetAsync(W.slot_hist.p, 0, (size_t)d->n_cslots * 8, st), "memset slot counts")) ||
+                !cuda_ok(cudaMemsetAsync(W.rec_hist.p, 0, (size_t)d->n_outputs * 8, st), "memset record counts"))
+                return DACH_CUDA_ERROR;
+            P.slot_hist = static_cast<unsigned long long*>(W.slot_hist.p);
+            P.rec_hist = static_cast<unsigned long long*>(W.rec_hist.p);
+            P.hist_smem = hist_k;
+        }
+        const size_t smem = plan_smem(d, P, machine, std3, threads, ctas_per_sm, 1, hist_k);
         k_check_offsets<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_offs, n, (uint64_t)(text_end - d_text), P.ctrl);
         ++d->launches;
         if (seg) enqueue_seg_table(d, W, d_offs, n, seg_len, 0, P, st);
         cudaEventRecord(W.ev[3], st);
         const int which = std3 ? 3 : machine ? 1 : 0;
         const int t = machine ? std::min(threads, 1024) : threads;
-        if (!cuda_ok(rk == RK_COUNT ? launch_rk<RK_COUNT>(which, d->charwise, mmode, P, grid, t, smem, st)
-                                    : launch_rk<RK_FIRST>(which, d->charwise, mmode, P, grid, t, smem, st),
+        if (!cuda_ok(rk == RK_COUNT  ? launch_rk<RK_COUNT>(which, d->charwise, mmode, P, grid, t, smem, st)
+                     : rk == RK_HIST ? launch_rk<RK_HIST>(which, d->charwise, mmode, P, grid, t, smem, st)
+                                     : launch_rk<RK_FIRST>(which, d->charwise, mmode, P, grid, t, smem, st),
                      "k_scan launch"))
             return DACH_CUDA_ERROR;
         cudaEventRecord(W.ev[1], st);
         const unsigned long long* seg_first = seg ? static_cast<const unsigned long long*>(W.seg_first.p) : nullptr;
-        if (rk == RK_COUNT)
+        if (rk == RK_HIST) {
+            // lane machines: slot counts -> head records; an event of find_overlapping reports the head's whole list
+            if (machine) {
+                k_hist_heads<<<(unsigned)std::max<uint64_t>(1, std::min<uint64_t>((d->n_cslots + 255) / 256, 8 * d->sm_count)), 256, 0, st>>>(
+                    P.slot_hist, d->d_opos, d->n_cslots, P.rec_hist);
+                ++d->launches;
+            }
+            const unsigned fb = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((d->n_outputs + 255) / 256, 8 * d->sm_count));
+            unsigned long long* hist = reinterpret_cast<unsigned long long*>(d_hist);
+            if (machine && mmode == M_OVERLAPPING)
+                k_hist_fold<true><<<fb, 256, 0, st>>>(P.rec_hist, d->d_outputs, d->n_outputs, key, hist, total);
+            else
+                k_hist_fold<false><<<fb, 256, 0, st>>>(P.rec_hist, d->d_outputs, d->n_outputs, key, hist, total);
+            ++d->launches;
+        } else if (rk == RK_COUNT)
             k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(d_counts), total);
         else
             k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(d_first), d_found, total);
-        d->launches += 2;
+        if (rk != RK_HIST) d->launches += 2;  // the scan and k_count_hay / k_first_hay
+        else ++d->launches;                   // the scan
         if (!cuda_ok(cudaGetLastError(), "kernel launch")) return DACH_CUDA_ERROR;
     } else {
         cudaEventRecord(W.ev[1], st);
@@ -1838,6 +1923,85 @@ int rk_batch_host_impl(dach_dev* d, int rk, int mode, const uint8_t* text, const
     return DACH_OK;
 }
 
+// HIST: the key and the size of the caller's histogram, decided before anything is launched
+int check_hist(const dach_dev* d, int key, uint64_t n_hist) {
+    if (key != DACH_KEY_OUTPUT && key != DACH_KEY_VALUE) {
+        set_error("unknown histogram key");
+        return DACH_INVALID_ARGUMENT;
+    }
+    if (key == DACH_KEY_OUTPUT ? n_hist < d->n_outputs : (d->n_outputs && n_hist <= d->max_value)) {
+        set_error(key == DACH_KEY_OUTPUT ? "n_hist is below the number of output records"
+                                         : "n_hist must exceed the largest pattern value");
+        return DACH_INVALID_ARGUMENT;
+    }
+    return DACH_OK;
+}
+
+// HIST of a host-buffer batch: the slices of dach_scan_batch_host add into one device histogram, which comes back once
+// and is added into the caller's
+int hist_batch_host_impl(dach_dev* d, int mode, int key, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* hist,
+                         uint64_t n_hist, uint64_t* total) {
+    if (!d || !offs || (n_hist && !hist)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    int rc = check_hist(d, key, n_hist);
+    if (rc) return rc;
+    rc = check_mode(d, mode);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(d->mu);
+    DeviceGuard g(d->device);
+    if (!g.ok) return DACH_CUDA_ERROR;
+    d->last_h2d = d->last_d2h = 0;
+    if (total) *total = 0;
+    if (n == 0) return DACH_OK;
+    rc = check_host_offsets(offs, n);
+    if (rc) return rc;
+    struct Drain {  // no exit may leave copies of the caller's buffers in flight
+        dach_dev* d;
+        ~Drain() {
+            for (Workspace& w : d->slot)
+                if (w.stream) cudaStreamSynchronize(w.stream);
+        }
+    } drain_on_exit{d};
+    const std::vector<Slice> slices = cut_slices(d, mode, offs, n);
+    for (Workspace& w : d->slot)
+        if (!w.init(true)) return DACH_CUDA_ERROR;
+    // the batch's histogram: zeroed before any slice adds into it (the slices run on the slots' streams)
+    DevBuf& acc = d->slot[0].hist_acc;
+    if (!ensure(acc, n_hist * 8) || !cuda_ok(cudaMemsetAsync(acc.p, 0, n_hist * 8, d->slot[0].stream), "memset histogram") ||
+        !cuda_ok(cudaStreamSynchronize(d->slot[0].stream), "memset histogram"))
+        return DACH_CUDA_ERROR;
+    double t_reuse = 0;
+    auto issue_h2d = [&](size_t k) -> bool {
+        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
+    };
+    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
+    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
+    uint64_t sum = 0;
+    for (size_t k = 0; k < slices.size(); ++k) {
+        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
+        Workspace& W = d->slot[k % dach_dev::kSlots];
+        const Slice& s = slices[k];
+        const uint64_t tb = offs[s.last] - offs[s.first], ns = s.last - s.first;
+        const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
+        rc = enqueue_rk(d, W, RK_HIST, mode, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb, tb,
+                        static_cast<const uint64_t*>(W.offs.p), ns, nullptr, nullptr, nullptr, W.stream, key, static_cast<uint64_t*>(acc.p));
+        uint64_t t = 0;
+        if (!rc) rc = finish_rk(d, W, &t);
+        if (rc) return rc;
+        sum += t;
+    }
+    for (Workspace& w : d->slot)
+        if (!cuda_ok(cudaStreamSynchronize(w.stream), "scan")) return DACH_CUDA_ERROR;
+    std::vector<uint64_t> h(n_hist);
+    if (n_hist && !cuda_ok(cudaMemcpy(h.data(), acc.p, n_hist * 8, cudaMemcpyDeviceToHost), "D2H histogram")) return DACH_CUDA_ERROR;
+    d->last_d2h = n_hist * 8;
+    for (uint64_t i = 0; i < n_hist; ++i) hist[i] += h[i];
+    if (total) *total = sum;
+    return DACH_OK;
+}
+
 // maps every exception to a status: nothing may unwind through the C ABI
 template <class F>
 int guarded(F&& f) {
@@ -1888,6 +2052,9 @@ int dach_dev_upload(const dach_pma* pma, int device, dach_dev** out) {
         d->max_pattern_len = img.max_pattern_len;
         d->segmentable = img.segmentable;
         d->mapper_len = (uint32_t)img.mapper.size();
+        d->n_outputs = (uint32_t)(img.outputs.size() / 4);
+        for (uint32_t i = 0; i < d->n_outputs; ++i) d->max_value = std::max(d->max_value, img.outputs[(size_t)i * 4]);
+        d->n_cslots = (uint32_t)img.opos_tab.size();
         cudaDeviceProp prop;
         if (!cuda_ok(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties")) return DACH_CUDA_ERROR;
         d->sm_count = prop.multiProcessorCount;
@@ -2036,6 +2203,31 @@ int dach_dev_first_batch(dach_dev* d, int mode, const uint8_t* d_text, const uin
 int dach_first_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, dach_match* first, uint8_t* found,
                           uint64_t* n_found) {
     return guarded([&]() -> int { return rk_batch_host_impl(d, RK_FIRST, mode, text, offs, n, nullptr, first, found, n_found); });
+}
+
+int dach_dev_hist_batch(dach_dev* d, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                        uint64_t* d_hist, uint64_t n_hist, uint64_t* total, void* stream) {
+    if (!d || !d_offs || (n_hist && !d_hist)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    int rc = check_hist(d, key, n_hist);
+    if (rc) return rc;
+    rc = check_mode(d, mode);
+    if (rc) return rc;
+    return guarded([&]() -> int {
+        std::lock_guard<std::mutex> lk(d->mu);
+        DeviceGuard g(d->device);
+        if (!g.ok) return DACH_CUDA_ERROR;
+        const int r = enqueue_rk(d, d->ws, RK_HIST, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, nullptr, nullptr,
+                                 nullptr, static_cast<cudaStream_t>(stream), key, d_hist);
+        return r ? r : finish_rk(d, d->ws, total);
+    });
+}
+
+int dach_hist_batch_host(dach_dev* d, int mode, int key, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* hist,
+                         uint64_t n_hist, uint64_t* total) {
+    return guarded([&]() -> int { return hist_batch_host_impl(d, mode, key, text, offs, n, hist, n_hist, total); });
 }
 
 // ---- asynchronous jobs ------------------------------------------------------------------------------
@@ -2425,6 +2617,8 @@ int dach_dev_set_option(dach_dev* d, const char* name, int64_t value) {
         d->opt_smem_pad_kib = value;
     else if (k == "hot_entries")
         d->opt_hot_entries = value;
+    else if (k == "hist_smem")
+        d->opt_hist_smem = value;
     else if (k == "l2_hints") {
         d->opt_l2_hints = value;
         DeviceGuard g(d->device);

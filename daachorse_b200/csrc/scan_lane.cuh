@@ -16,8 +16,8 @@
 //   - StdMachine3  the default (kernel=3): no probe-state flags, one stop bit, cursor = address word, records from
 //                  the hot-first image (optionally its front from shared memory); probe / resolve are separate so
 //                  that k_scan_duo can keep two fetches in flight; serves stream chunks
-//   - SinkOps      COUNT / FIRST on StdMachine3, LmMachine, CwMachine: their drain() / begin_item() for the
-//                  other result kinds (sinks: Emitter, CountSink, FirstSink)
+//   - SinkOps      COUNT / FIRST / HIST on StdMachine3, LmMachine, CwMachine: their drain() / begin_item() for
+//                  the other result kinds (sinks: Emitter, CountSink, FirstSink, HistSink)
 //
 // Device image (built by dev_image.cpp from the validated host automaton):
 //   wide bytewise record  uint4 {base, efail, fbase, opos<<8 | check}      16 B / slot
@@ -141,12 +141,18 @@ struct ScanParams {
     // results of the other result kinds (CountSink / FirstSink), per item
     unsigned long long* item_count;
     uint4* item_first;  // {start, end, value, found}
+    // HIST (HistSink): events per compact slot (lane machines) / reported matches per output record (lane per
+    // haystack), and how many leading compact slots count in shared memory first
+    unsigned long long* slot_hist;
+    unsigned long long* rec_hist;
+    uint32_t hist_smem;
 };
 
-// What a scan produces (compile time): every match (Emitter), the number of matches (CountSink), or the first
-// match and whether there is one (FirstSink).  The lane machines and the lane-per-haystack loops are the same
-// for all three; the sink and, for FIRST, the stop rule differ.
-constexpr int RK_MATCHES = 0, RK_COUNT = 1, RK_FIRST = 2;
+// What a scan produces (compile time): every match (Emitter), the number of matches (CountSink), the first
+// match and whether there is one (FirstSink), or the matches per output record of the whole batch (HistSink).
+// The lane machines and the lane-per-haystack loops are the same for all four; the sink and, for FIRST, the
+// stop rule differ.
+constexpr int RK_MATCHES = 0, RK_COUNT = 1, RK_FIRST = 2, RK_HIST = 3;
 
 // L2 eviction policies (64-bit descriptors made once per device by k_make_policies, dev_scan.cu):
 //   [0] automaton image (records, output_pos, outputs, mapper): evict_last -- the scan is latency-bound on
@@ -362,6 +368,63 @@ DACH_HD void emit_chain(const ScanParams& P, FirstSink& E, uint32_t opos, uint32
     if (opos != 0) emit_head(P, E, opos, end);
 }
 
+// *p += v with no return value (red.global.add.u64)
+DACH_HD void red_add_u64(unsigned long long* p, unsigned long long v) {
+#if defined(__CUDA_ARCH__)
+    asm volatile("red.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+#else
+    *p += v;
+#endif
+}
+
+// HIST: occurrences per output record over the whole batch, nothing per item.
+//   lane machines: event(slot) counts the event's state -- for find_overlapping the event stands for the
+//       state's whole list, for the other iterators for its head -- in P.slot_hist; the post-passes of
+//       dev_scan.cu (k_hist_heads, k_hist_fold) give every record its count.  Slots below `k` count in
+//       CTA-private u32 counters in shared memory first (`s_cnt`, flushed once when the CTA ends): the
+//       hot-first layout puts the shallowest states, where most events land, at the front.  A counter that
+//       reaches 2^31 hands 2^31 on to global memory at once (the one thread whose increment crossed it), so
+//       it would take 2^31 more increments of the same counter before that thread's next instruction to
+//       overflow it.
+//   lane per haystack: emit_head / emit_chain add 1 per reported match to its record in P.rec_hist.
+struct HistSink {
+    static constexpr int KIND = RK_HIST;
+    unsigned int* s_cnt = nullptr;
+    uint32_t k = 0;
+    uint32_t item = 0;
+    DACH_HD void begin(uint32_t item_id) { item = item_id; }
+    DACH_HD void finish(const ScanParams&) {}
+    DACH_HD bool stopped() const { return false; }
+    // a match known by its value alone cannot be counted per record: scan_standard routes ROOT's matches
+    // through emit_head for HIST, so this is never reached
+    DACH_HD void emit(const ScanParams&, uint32_t, uint32_t, uint32_t) {}
+    DACH_HD void event(const ScanParams& P, uint32_t slot) {
+        if (slot < k) {
+#if defined(__CUDA_ARCH__)
+            const unsigned int old = atomicAdd(s_cnt + slot, 1u);
+            if (old == 0x7fffffffu) {
+                atomicSub(s_cnt + slot, 0x80000000u);
+                red_add_u64(P.slot_hist + slot, 0x80000000ull);
+            }
+#else
+            if (++s_cnt[slot] == 0x80000000u) {
+                s_cnt[slot] = 0;
+                red_add_u64(P.slot_hist + slot, 0x80000000ull);
+            }
+#endif
+        } else {
+            red_add_u64(P.slot_hist + slot, 1);
+        }
+    }
+};
+DACH_HD void emit_head(const ScanParams& P, HistSink&, uint32_t opos, uint32_t) { red_add_u64(P.rec_hist + (opos - 1), 1); }
+DACH_HD void emit_chain(const ScanParams& P, HistSink&, uint32_t opos, uint32_t) {
+    while (opos != 0) {
+        red_add_u64(P.rec_hist + (opos - 1), 1);
+        opos = ld_u4(P.outputs + (opos - 1)).z;
+    }
+}
+
 // ---- record access: leading `hot_n` records come from shared memory --------------------
 struct RecView {
     const uint4* glob;
@@ -485,8 +548,25 @@ DACH_HD void scan_standard(const ScanParams& P, const RecView& V, TextWin& T, SI
     if (CHARWISE) root_rec = V.get(D_ROOT);
     if (MODE == M_OVERLAPPING) emit_chain(P, E, root_opos, 0);
     if (MODE == M_NO_SUFFIX && root_opos) {
-        const uint4 o = ld_u4(P.outputs + (root_opos - 1));
-        E.emit(P, 0, 0, o.x);  // length 0, end 0 (iter.rs:210-214)
+        if constexpr (SINK::KIND == RK_HIST) {
+            emit_head(P, E, root_opos, 0);
+        } else {
+            const uint4 o = ld_u4(P.outputs + (root_opos - 1));
+            E.emit(P, 0, 0, o.x);  // length 0, end 0 (iter.rs:210-214)
+        }
+    }
+    if constexpr (SINK::KIND == RK_HIST) {
+        if (MODE == M_FIND && root_opos) {  // one match of ROOT's record per boundary
+            unsigned long long k = 1;
+            for (uint32_t pos = 0; pos < len; ++k) {
+                if (CHARWISE)
+                    (void)utf8_at(T, pos);
+                else
+                    ++pos;
+            }
+            red_add_u64(P.rec_hist + (root_opos - 1), k);
+            return;
+        }
     }
     if (MODE == M_FIND && root_opos) {
         // an empty pattern exists: only zero-length matches, one per boundary (iter.rs:60-85)
@@ -2048,12 +2128,15 @@ struct StdMachine3 {
 //          first event fills it and the machine stops by its own rule.  If the event is reportable (it
 //          ends inside the item's segment; warm-up events do not count) its list head is the item's
 //          answer and the item is done; otherwise the queue is emptied and the lane goes on.
+//   HIST   adds 1 per reportable event to the event's slot (HistSink::event): no output list is read
+//          here; dev_scan.cu's post-passes turn slot counts into output-record counts.
 // MODE is the machine's iterator: FIRST of a Standard automaton always runs the find_overlapping
 // machine, whose first event is the first event of all three Standard iterators.
 // =============================================================================================
 template <class M, int MODE, int RK>
 struct SinkOps {
-    using Sink = typename std::conditional<RK == RK_COUNT, CountSink, FirstSink>::type;
+    using Sink = typename std::conditional<RK == RK_COUNT, CountSink,
+                                           typename std::conditional<RK == RK_FIRST, FirstSink, HistSink>::type>::type;
 
     template <class LANE>
     static DACH_HD void begin_item(LANE& L, const ScanParams& P, const StdEnv& Ev, Sink& E, uint64_t item, const uint8_t* emu_lo) {
@@ -2078,6 +2161,14 @@ struct SinkOps {
                 if (j < L.qn) {
                     const QEntry e = Ev.q[j * Ev.q_stride];
                     if (e.end >= L.from) E.count += MODE == M_OVERLAPPING ? chain_len(P, ld_u32(Ev.opos + e.opos)) : 1u;
+                }
+            }
+            L.qn = 0;
+        } else if constexpr (RK == RK_HIST) {
+            for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j) {
+                if (j < L.qn) {
+                    const QEntry e = Ev.q[j * Ev.q_stride];
+                    if (e.end >= L.from) E.event(P, e.opos);  // the entry holds the slot
                 }
             }
             L.qn = 0;

@@ -112,6 +112,14 @@ size_t dach_pma_heap_bytes(const dach_pma *pma);
 size_t dach_pma_num_elements(const dach_pma *pma);
 int dach_pma_is_charwise(const dach_pma *pma);
 uint32_t dach_pma_max_pattern_len(const dach_pma *pma); /* longest pattern in bytes */
+/* The output records (src/nfa_builder.rs:203-222): one per pattern the builder kept -- duplicates get
+ * a record each; LeftmostFirst drops patterns that extend a shorter one.  dach_pma_outputs copies
+ * record i's value, length (bytes) and parent (0 = none, else the parent's 1-based index; a parent
+ * comes before its child) to values[i] / lengths[i] / parents[i]; any array may be NULL.
+ * n < dach_pma_num_outputs -> DACH_INVALID_ARGUMENT.  These label DACH_KEY_OUTPUT histograms. */
+uint32_t dach_pma_num_outputs(const dach_pma *pma);
+int dach_pma_outputs(const dach_pma *pma, uint32_t *values, uint32_t *lengths, uint32_t *parents,
+                     uint32_t n);
 void dach_pma_free(dach_pma *pma);
 
 /* ---- device image ---------------------------------------------------------------- */
@@ -202,6 +210,34 @@ int dach_dev_first_batch(dach_dev *dev, int mode, const uint8_t *d_text, const u
                          uint64_t text_bytes, dach_match *d_first, uint8_t *d_found, uint64_t *n_found, void *stream);
 int dach_first_batch_host(dach_dev *dev, int mode, const uint8_t *text, const uint64_t *offs, uint64_t n,
                           dach_match *first, uint8_t *found, uint64_t *n_found);
+
+/* ---- per-pattern occurrence counts ------------------------------------------------------------
+ *
+ * How often each pattern occurs in a batch, with no match list: hist[k] += the number of matches
+ * iterator `mode` yields over all n haystacks whose key is k.
+ *   DACH_KEY_OUTPUT  k = the index of the match's output record (dach_pma_outputs); n_hist must be at
+ *                    least dach_pma_num_outputs.
+ *   DACH_KEY_VALUE   k = the match's value: exactly a bincount of the values of dach_dev_scan_batch.
+ *                    n_hist must exceed the largest value.  For automata made by `new` the value is the
+ *                    pattern index.
+ * The counts are ADDED into the caller's zeroed (or earlier) histogram, so calls on batches A and B
+ * leave what one call on A ++ B would: a corpus accumulates on the device across batches (and across
+ * GPUs with an ordinary all-reduce).  *total = the matches added (== the dach_dev_count_batch total).
+ * A too-small n_hist or an unknown key is DACH_INVALID_ARGUMENT before anything runs; offsets, modes
+ * and the missing device as dach_dev_count_batch.  The calls synchronise `stream`.
+ * The host form uses the slices of dach_scan_batch_host, adds them up on the device and copies
+ * n_hist x 8 bytes back once (dach_dev_last_d2h_bytes).  Option hist_smem (default 1024; 0 = off):
+ * events of the leading compact states are counted in shared memory per CTA first.  Options kernel and
+ * the fallbacks as dach_dev_count_batch.  Stream chunks, jobs and shard groups have no histogram form. */
+typedef enum {
+    DACH_KEY_OUTPUT = 0,
+    DACH_KEY_VALUE = 1
+} dach_hist_key;
+int dach_dev_hist_batch(dach_dev *dev, int mode, int key, const uint8_t *d_text, const uint64_t *d_offs,
+                        uint64_t n, uint64_t text_bytes, uint64_t *d_hist, uint64_t n_hist, uint64_t *total,
+                        void *stream);
+int dach_hist_batch_host(dach_dev *dev, int mode, int key, const uint8_t *text, const uint64_t *offs,
+                         uint64_t n, uint64_t *hist, uint64_t n_hist, uint64_t *total);
 
 /* ---- asynchronous scans (jobs) ----------------------------------------------------------
  *

@@ -45,6 +45,10 @@ pub const DACH_FIND_OVERLAPPING: i32 = 1; // find_overlapping_iter           src
 pub const DACH_FIND_OVERLAPPING_NO_SUFFIX: i32 = 2; // find_overlapping_no_suffix_iter src/bytewise.rs:410
 pub const DACH_LEFTMOST_FIND: i32 = 3; // leftmost_find_iter              src/bytewise.rs:547
 
+// histogram keys (dach_dev_hist_batch)
+pub const DACH_KEY_OUTPUT: i32 = 0; // index of the match's output record (dach_pma_outputs)
+pub const DACH_KEY_VALUE: i32 = 1; // the match's value
+
 #[link(name = "daachorse_b200")]
 extern "C" {
     pub fn dach_abi_version() -> i32;
@@ -55,6 +59,9 @@ extern "C" {
     pub fn dach_pma_deserialize(src: *const u8, len: usize, charwise: i32, out: *mut *mut DachPma,
                                 consumed: *mut usize) -> i32;
     pub fn dach_pma_free(pma: *mut DachPma);
+    /// The output records (src/nfa_builder.rs:203-222): values / lengths / parents (0 = none, else 1-based).
+    pub fn dach_pma_num_outputs(pma: *const DachPma) -> u32;
+    pub fn dach_pma_outputs(pma: *const DachPma, values: *mut u32, lengths: *mut u32, parents: *mut u32, n: u32) -> i32;
 
     pub fn dach_dev_upload(pma: *const DachPma, device: i32, out: *mut *mut DachDev) -> i32;
     pub fn dach_dev_free(dev: *mut DachDev);
@@ -74,6 +81,12 @@ extern "C" {
     pub fn dach_dev_first_batch(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
                                 text_bytes: u64, d_first: *mut DachMatch, d_found: *mut u8, n_found: *mut u64,
                                 stream: *mut c_void) -> i32;
+    /// Occurrences per key over the batch, ADDED into hist[0..n_hist) (key: DACH_KEY_OUTPUT / DACH_KEY_VALUE);
+    /// *total = the matches added.  n_hist below the record count / not above the largest value: DACH_INVALID_ARGUMENT.
+    pub fn dach_hist_batch_host(dev: *mut DachDev, mode: i32, key: i32, text: *const u8, offs: *const u64, n: u64,
+                                hist: *mut u64, n_hist: u64, total: *mut u64) -> i32;
+    pub fn dach_dev_hist_batch(dev: *mut DachDev, mode: i32, key: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                               text_bytes: u64, d_hist: *mut u64, n_hist: u64, total: *mut u64, stream: *mut c_void) -> i32;
     /// Device-resident buffers.
     pub fn dach_dev_scan_batch(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
                                text_bytes: u64, d_out: *mut DachMatch, out_cap: u64, d_out_offs: *mut u64,

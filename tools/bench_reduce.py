@@ -3,9 +3,10 @@
 
     python tools/bench_reduce.py --output counts [--config C3|C3-find|C2|C4|C5] [--steps K] [--warmup W]
     python tools/bench_reduce.py --output first  ...
+    python tools/bench_reduce.py --output hist [--key value|output] ...
 
-One step = one dach_dev_count_batch / dach_dev_first_batch on the step's batch (the batches, automata and seeds of
-bench.py).  One JSON line, bench.py's fields where they apply:
+One step = one dach_dev_count_batch / dach_dev_first_batch / dach_dev_hist_batch on the step's batch (the batches,
+automata and seeds of bench.py).  One JSON line, bench.py's fields where they apply:
   value              bytes offered / device time of the call's pipeline (CUDA events inside the library)
   roofline           bench.py's definition, on the COUNT / FIRST scan kernel
   e2e                the same batch through dach_count_batch_host / dach_first_batch_host from pinned host text
@@ -14,6 +15,10 @@ bench.py).  One JSON line, bench.py's fields where they apply:
                      matches scan of the same batch
   first_end_frac     (first) mean first.end / haystack length over the haystacks with a match: how much of what it
                      is offered FIRST reads
+  alternatives       (hist) in the same run, GB/s by CUDA events around whole steps: the histogram call, the full
+                     matches scan (dach_dev_scan_batch) + torch.bincount of the values, and COUNT; the hist parity
+                     checks the value-keyed histogram against np.bincount of the oracle sample's values, and the whole
+                     step against the full scan bincounted on the device
   launches_per_step  kernels launched per step
 Nothing is written to the tree.
 """
@@ -42,6 +47,15 @@ def reduce_parity(output, got_counts, got_first, got_found, ref_counts, ref_firs
     k = len(ref_first)
     return {"found_equal": bool(np.array_equal(got_found.astype(bool), ref_found.astype(bool))),
             "first_equal": got_first[:k].astype(np.uint32).tobytes() == ref_first.astype(np.uint32).tobytes()}
+
+
+def hist_parity(got_hist, ref_values, n_hist):
+    """In-run parity of --output hist (value key) on the oracle sample: the histogram against np.bincount of the
+    oracle's match values, and its total against their number."""
+    ref = np.bincount(np.asarray(ref_values, dtype=np.int64), minlength=n_hist).astype(np.uint64)
+    got = np.asarray(got_hist).astype(np.uint64)
+    return {"hist_equal": bool(len(got) == len(ref) and np.array_equal(got, ref)),
+            "total_equal": int(got.sum()) == int(len(ref_values))}
 
 
 def first_from_matches(matches, counts):
@@ -74,6 +88,8 @@ def run_reduce_output(args, W, pma, batches, dmode, omode, n, hay_len, step_byte
     import torch
 
     setup_s = time.time() - t_setup
+    if args.output == "hist":
+        return run_hist_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s)
     counts_t = torch.empty(n, dtype=torch.int64, device=dev)
     first_t = torch.empty((n, 3), dtype=torch.int32, device=dev)
     found_t = torch.empty(n, dtype=torch.bool, device=dev)
@@ -182,9 +198,151 @@ def run_reduce_output(args, W, pma, batches, dmode, omode, n, hay_len, step_byte
     }
 
 
+def _card():
+    import subprocess
+
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=20).stdout.strip()
+        name, plim = [x.strip() for x in q.split(",")[:2]]
+        return {"name": name, "power_limit": plim}
+    except Exception:
+        import torch
+
+        return {"name": torch.cuda.get_device_name(0), "power_limit": None}
+
+
+def run_hist_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s):
+    """--output hist: every step is one dach_dev_hist_batch on the step's batch, added into one device histogram (the
+    additive contract: a corpus accumulates).  The same run times the full matches scan + torch.bincount of its values
+    and COUNT on the same batches, step by step, by CUDA events around whole steps."""
+    import torch
+
+    vals = pma.outputs()[0]
+    n_hist = (int(vals.max()) + 1 if len(vals) else 0) if args.key == "value" else len(vals)
+    hist_t = torch.zeros(n_hist, dtype=torch.int64, device=dev)
+    counts_t = torch.empty(n, dtype=torch.int64, device=dev)
+    r0 = pma.scan_batch_device(dmode, *batches[0])
+    cap = int(max(r0.matches.shape[0], 1) * 1.25) + 1024
+    del r0
+    out_m = torch.empty((cap, 3), dtype=torch.int32, device=dev)
+    out_o = torch.empty(n + 1, dtype=torch.int64, device=dev)
+
+    def hist_step(s):
+        t, o = batches[s % len(batches)]
+        pma.pattern_counts_device(dmode, t, o, key=args.key, out=hist_t)
+        st = pma.stats()
+        return st["scan_kernel_ms"], st["total_ms"]
+
+    def matches_step(s):
+        t, o = batches[s % len(batches)]
+        r = pma.scan_batch_device(dmode, t, o, out=out_m, out_offs=out_o)
+        return torch.bincount(r.matches[:, 2].long(), minlength=n_hist)
+
+    def count_step(s):
+        t, o = batches[s % len(batches)]
+        pma.count_batch_device(dmode, t, o, out=counts_t)
+
+    def timed(fn):
+        for s in range(args.warmup):
+            fn(s)
+        torch.cuda.synchronize()
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+        res = [fn(args.warmup + s) for s in range(args.steps)]
+        ev1.record()
+        torch.cuda.synchronize()
+        return ev0.elapsed_time(ev1) / args.steps, res
+
+    sampler = ClockSampler(dev.index)
+    sampler.start()
+    time.sleep(0.2)
+    n_before = len(sampler.rows)
+    launches1 = pma.stats()["launches"]
+    hist_ms, times = timed(hist_step)
+    launches2 = pma.stats()["launches"]
+    matches_ms, _ = timed(matches_step)
+    count_ms, _ = timed(count_step)
+    time.sleep(0.25)
+    clocks = sampler.stop(skip=n_before)
+    k_ms = float(np.mean([t[0] for t in times]))
+    dev_ms = float(np.mean([t[1] for t in times]))
+    value = step_bytes / (dev_ms * 1e-3) / 1e9
+    gbs = lambda ms: step_bytes / (ms * 1e-3) / 1e9  # noqa: E731
+    # the whole last step against the full scan of the same batch, bincounted on the device
+    last_batch = (args.warmup + args.steps - 1) % len(batches)
+    t_last, o_last = batches[last_batch]
+    one = pma.pattern_counts_device(dmode, t_last, o_last, key=args.key)
+    r = pma.scan_batch_device(dmode, t_last, o_last)
+    full = torch.bincount(r.matches[:, 2].long(), minlength=int(vals.max()) + 1 if len(vals) else 0)
+    if args.key == "output":
+        full = full[torch.from_numpy(vals.astype(np.int64)).to(dev)]  # new(): one value per record
+    step_ok = bool(torch.equal(one, full))
+    total = int(one.sum().item())
+    del r, full
+    parity = None
+    if not args.no_cpu:
+        import oracle_api as O
+
+        threads = O.cpu_budget()["threads"]
+        ns = max(1, min(n, int(n * args.parity_frac)))
+        opma = W.oracle()
+        lo = W.batch_ranges()[last_batch][0]
+        ptext, poffs = W.host_batch(lo, lo + ns)
+        ref = opma.scan_batch(omode, ptext, poffs, nthreads=threads, want_matches=True)
+        nv = int(vals.max()) + 1 if len(vals) else 0
+        got = pma.pattern_counts_host(dmode, ptext, poffs, key="value")
+        parity = hist_parity(got, ref["matches"]["value"], nv)
+        parity.update({"haystacks_checked": ns, "share_of_batch": ns / n,
+                       "what": "value-keyed histogram of the first %d haystacks of the last batch vs np.bincount of the "
+                               "oracle's match values" % ns})
+    parity = dict(parity or {}, step_equals_full_scan=step_ok)
+    e2e = None
+    if not args.no_e2e:
+        t0_, o0_ = batches[0]
+        h_text_t = torch.empty(t0_.numel(), dtype=torch.uint8).pin_memory()
+        h_text_t.copy_(t0_)
+        h_text = h_text_t.numpy()
+        h_offs = o0_.cpu().numpy().astype(np.uint64)
+        e2e_ms = []
+        for i in range(1 + args.e2e_steps):
+            t0 = time.perf_counter()
+            pma.pattern_counts_host(dmode, h_text, h_offs, key=args.key)
+            if i >= 1:
+                e2e_ms.append((time.perf_counter() - t0) * 1e3)
+        st = pma.stats()
+        e2e = {"value": h_text.size / (np.mean(e2e_ms) * 1e-3) / 1e9, "unit": UNIT, "h2d_bytes_per_step": int(st["h2d_bytes"]),
+               "d2h_bytes_per_step": int(st["d2h_bytes"]), "ms_per_step": float(np.mean(e2e_ms)),
+               "workload": "the step batch's %d haystacks x %d B through the host entry point: pinned host text -> device -> "
+                           "scan -> one histogram of %d x 8 B to the host" % (n, hay_len, n_hist)}
+        del h_text_t
+    peak, peak_src = measured_peaks()
+    achieved = step_bytes / (k_ms * 1e-3) / 1e9
+    roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
+                "kernel": "k_scan_machine_rk (hist)", "kernel_ms": k_ms, "algorithmic_bytes_per_launch": step_bytes,
+                "peak_source": peak_src,
+                "note": "algorithmic bytes = 1 B read per haystack byte offered; kernel_ms = mean CUDA-event time of the scan kernel"}
+    return {
+        "metric": metric_name(W.spec) + ", hist (%s key)" % args.key, "output": "hist", "key": args.key, "value": value, "unit": UNIT,
+        "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": hist_ms, "device_ms_per_step": dev_ms,
+        "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
+        "config": {"workload": "%s: %s, %s, %d haystacks x %d B per step, %d batch(es) resident (%.2f GiB)" % (
+                       args.config, W.spec["what"], W.mode_name, n, hay_len, len(batches), resident / 2**30),
+                   "n_patterns": len(W.ps), "hay_len": hay_len, "bytes_per_gpu": step_bytes, "options": args.option,
+                   "setup_s": setup_s, "n_hist": n_hist},
+        "total": total,
+        "alternatives": {"unit": UNIT, "what": "CUDA events around %d whole steps each, same batches" % args.steps,
+                         "hist": gbs(hist_ms), "matches_plus_bincount": gbs(matches_ms), "count": gbs(count_ms),
+                         "hist_ms": hist_ms, "matches_plus_bincount_ms": matches_ms, "count_ms": count_ms},
+        "card": _card(), "roofline": roofline, "parity": parity, "e2e": e2e,
+        "gpu_launches": int(launches2 - launches1), "launches_per_step": (launches2 - launches1) / args.steps, "clocks": clocks,
+    }
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--output", required=True, choices=["counts", "first"])
+    ap.add_argument("--output", required=True, choices=["counts", "first", "hist"])
+    ap.add_argument("--key", default="value", choices=["value", "output"], help="--output hist: histogram key")
     ap.add_argument("--config", default="C3", choices=sorted(CONFIGS))
     ap.add_argument("--steps", type=int, default=None)
     ap.add_argument("--warmup", type=int, default=3)

@@ -1,7 +1,13 @@
 #!/usr/bin/env python3
 """Per-byte event counts of the bytewise Standard lane machine on samples of the bench workloads, from
 the CPU emulation of the kernels' lane code (tests/emu, StdMachine3 with its DACH_STAT counters).
-No GPU needed.  Usage: python tools/lane_stats.py [C2|C3|C5 ...]"""
+No GPU needed.  Usage: python tools/lane_stats.py [C2|C3|C5 ...]
+
+    python tools/lane_stats.py --events [C3 C3-find C2 C4 ...]
+
+reports instead how the lane machines' output events (what a HIST scan counts per state) spread over the compact
+slots: the share on the 1 / 64 / 1024 / 4096 busiest slots and on the leading 1024 / 4096 slots (what option hist_smem
+counts in shared memory), from tests/emu_hist."""
 import ctypes as C
 import os
 import sys
@@ -48,6 +54,35 @@ def need_cap(text):
     return len(text)  # >= 1 match per byte is far more than any config produces
 
 
+EVENT_CONFIGS = {"C3": ("C3", 1), "C3-find": ("C3", 0), "C2": ("C2", 1), "C4": ("C4", 3)}
+
+
+def event_shares(name, n_hay=256):
+    import emu_hist_api as H
+
+    synth, mode = EVENT_CONFIGS[name]
+    cfg = S.config(synth)
+    cw = cfg["variant"] == "charwise"
+    ps = S.make_patterns(cfg)
+    pool, b = S.make_pool(cfg, ps, 16 << 20)
+    kind = 1 if mode == 3 else 0  # C4: LeftmostLongest
+    opma = O.OraclePma.build_packed(ps.blob, ps.offs, charwise=cw, match_kind=kind)
+    hay_len = min(cfg["hay_len"], 1 << 14)
+    starts = S.window_starts(b, len(pool), n_hay, hay_len)
+    text, offs = S.materialise_host(pool, starts, hay_len)
+    if cw:
+        text = S.pad_to_char_boundary(text.reshape(n_hay, hay_len)).reshape(-1)
+    tops = [1, 64, 1024, 4096]
+    all_, top, lead = H.event_shares(opma.serialize(), cw, mode, text, offs, tops)
+    print("== %s: %d patterns, %d haystacks x %d B: %d events, %.4f per byte" % (name, len(ps), n_hay, hay_len, all_, all_ / len(text)))
+    print("   busiest slots:  " + "  ".join("top %d %.1f %%" % (k, 100.0 * top[k] / max(all_, 1)) for k in tops))
+    print("   leading slots:  " + "  ".join("< %d %.1f %%" % (k, 100.0 * lead[k] / max(all_, 1)) for k in tops[2:]))
+
+
 if __name__ == "__main__":
-    for nm in (sys.argv[1:] or ["C2", "C3"]):
-        run(nm)
+    if sys.argv[1:2] == ["--events"]:
+        for nm in (sys.argv[2:] or list(EVENT_CONFIGS)):
+            event_shares(nm)
+    else:
+        for nm in (sys.argv[1:] or ["C2", "C3"]):
+            run(nm)
