@@ -251,6 +251,18 @@ int build_image(const dach_pma* p, HostImage* img) {
         return DACH_INVALID_AUTOMATON;
     }
 
+    img->outputs.resize(p->outputs.size() * 4);
+    for (size_t i = 0; i < p->outputs.size(); ++i) {
+        img->outputs[i * 4 + 0] = p->outputs[i].value;
+        img->outputs[i * 4 + 1] = p->outputs[i].length;
+        img->outputs[i * 4 + 2] = p->outputs[i].parent;
+        // the length of the list that starts here (this record and its parents): what a count of
+        // find_overlapping adds per event without walking the list.  A parent comes before its child
+        // (deserialize checks parent < own 1-based index), so it is known already.
+        const uint32_t par = p->outputs[i].parent;
+        img->outputs[i * 4 + 3] = 1u + (par ? img->outputs[(size_t)(par - 1) * 4 + 3] : 0u);
+    }
+
     img->rec.resize(n * 4);
     if (!p->charwise) {
         auto skip_leaves = [&](uint32_t f) {  // failure target with child-less states skipped
@@ -317,7 +329,10 @@ int build_image(const dach_pma* p, HostImage* img) {
                 if (ns < H && R.vacant_check[ns]) check = R.vacant_check[ns] & 0xffu;  // ROOT, DEAD
                 r[0] = (R.new_base[s] << 8) | check;
                 r[1] = (nid(f) << 8) | flags;
-                r[2] = fbase << 8;
+                // low byte: the length of the state's output list, saturated at 255 (StdMachine3 queues it with
+                // the event, so that its drain needs neither output_pos nor the list)
+                const uint32_t list = opos ? img->outputs[(size_t)(opos - 1) * 4 + 3] : 0u;
+                r[2] = (fbase << 8) | std::min<uint32_t>(list, 255u);
                 r[3] = R.sig[s];
                 img->opos_tab[ns] = opos;
             }
@@ -377,17 +392,6 @@ int build_image(const dach_pma* p, HostImage* img) {
                 img->opos_tab[s] = p->output_pos[s];
             }
         }
-    }
-    img->outputs.resize(p->outputs.size() * 4);
-    for (size_t i = 0; i < p->outputs.size(); ++i) {
-        img->outputs[i * 4 + 0] = p->outputs[i].value;
-        img->outputs[i * 4 + 1] = p->outputs[i].length;
-        img->outputs[i * 4 + 2] = p->outputs[i].parent;
-        // the length of the list that starts here (this record and its parents): what a count of
-        // find_overlapping adds per event without walking the list.  A parent comes before its child
-        // (deserialize checks parent < own 1-based index), so it is known already.
-        const uint32_t par = p->outputs[i].parent;
-        img->outputs[i * 4 + 3] = 1u + (par ? img->outputs[(size_t)(par - 1) * 4 + 3] : 0u);
     }
     return DACH_OK;
 }

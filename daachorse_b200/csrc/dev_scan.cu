@@ -8,7 +8,8 @@
 //     k_scan_machine<M, LANE>   persistent grid (CTAs = SMs x ctas_per_sm); warps of 32 independent walkers pull
 //                               items from one atomic counter and step them in lock step through the automaton
 //                               image -- one record fetch per lane per iteration (scan_lane.cuh: StdMachine3,
-//                               LmMachine, CwMachine); matches go to pooled 256-byte blocks.
+//                               LmMachine, CwMachine); matches go to pooled 256-byte blocks -- StdMachine3 stores
+//                               its output events there as they are (event blocks), the others match tuples.
 //       k_scan_duo<MODE>        StdMachine3 with two haystacks per lane (option kernel = 4; measured slower)
 //       k_scan<CHARWISE, MODE>  lane per haystack, reference-shaped loop: automata above 2^24 slots, find_iter with
 //                               an empty pattern, and option kernel = 0
@@ -20,6 +21,7 @@
 //   phase 2
 //     k_gather                  every pooled block to its final place: dense, ordered exactly like the crate's
 //                               iterators, at a device-side base, into any buffer (the caller's, a job's packed copy)
+//     k_expand                  the same for event blocks: every event expanded into its output list's tuples
 //     k_final_offsets           the caller's per-haystack offsets (+ base)
 //     k_add_base                stream chunks: positions in stream coordinates
 //   shard groups (dach_group_place)
@@ -181,7 +183,21 @@ __device__ __forceinline__ void scan_machine(const ScanParams& P) {
     if (HOT) mbar_wait(&s_bar, 0);
     for (;;) {
         // ---- service phase (the warp is converged here) ----
-        if (L.fl & F_ACTIVE) OPS::drain(L, Ev, P, E);
+        if constexpr (std::is_same<SINK, EventSink>::value) {
+            // event blocks: the lanes that need one this phase take them with one atomic for the warp
+            const bool want = (L.fl & F_ACTIVE) && OPS::need_block(L, Ev, E);
+            const unsigned mb = __ballot_sync(FULL, want);
+            uint32_t blk = 0;
+            if (mb) {
+                const int leader = __ffs(mb) - 1;
+                unsigned int b0 = 0;
+                if ((int)lane == leader) b0 = atomicAdd(&P.ctrl->blk_cursor, (unsigned int)__popc(mb));
+                blk = __shfl_sync(FULL, b0, leader) + __popc(mb & ((1u << lane) - 1u));
+            }
+            if (L.fl & F_ACTIVE) OPS::drain(L, Ev, P, E, blk);
+        } else {
+            if (L.fl & F_ACTIVE) OPS::drain(L, Ev, P, E);
+        }
         if ((L.fl & (F_ACTIVE | F_DONE)) == (F_ACTIVE | F_DONE)) {
             E.finish(P);
             M::finish_item(L, P);
@@ -240,9 +256,13 @@ __device__ __forceinline__ void scan_machine(const ScanParams& P) {
     }
 }
 
+// matches: StdMachine3 stores events (EventOps, expanded by k_expand), the other machines match tuples (k_gather)
 template <class M, class LANE, int MAXT, int MINB, bool HOT>
 __global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
-    scan_machine<M, M, LANE, Emitter, HOT>(P);
+    if constexpr (M::QLEN)
+        scan_machine<M, EventOps<M::ITER>, LANE, EventSink, HOT>(P);
+    else
+        scan_machine<M, M, LANE, Emitter, HOT>(P);
 }
 // COUNT / FIRST (result kind RK) on the lane machine M running iterator MODE
 template <class M, class LANE, int MODE, int RK, bool HOT>
@@ -379,20 +399,20 @@ __device__ __forceinline__ unsigned long long block_exclusive_scan(unsigned long
     return before + inc - v;
 }
 
-// BLOCKS: scan ceil(count / BLK_MATCHES) (pool blocks per item) instead of the counts themselves
-template <bool BLOCKS>
+// PER > 1: scan ceil(count / PER) (pool blocks per item, PER entries a block) instead of the counts themselves
+template <uint32_t PER>
 __device__ __forceinline__ uint32_t scan_term(uint32_t count) {
-    return BLOCKS ? (count + BLK_MATCHES - 1) / BLK_MATCHES : count;
+    return PER > 1 ? (count + PER - 1) / PER : count;
 }
 
-template <bool BLOCKS>
+template <uint32_t PER>
 __global__ void __launch_bounds__(kScanThreads) k_offsets_tile_sums(const uint32_t* counts, uint64_t n,
                                                                       unsigned long long* tile_sums) {
     const uint64_t base = (uint64_t)blockIdx.x * kScanTile;
     unsigned long long s = 0;
     for (int k = 0; k < kScanPerThread; ++k) {
         const uint64_t i = base + (uint64_t)k * kScanThreads + threadIdx.x;
-        if (i < n) s += scan_term<BLOCKS>(counts[i]);
+        if (i < n) s += scan_term<PER>(counts[i]);
     }
     unsigned long long total;
     (void)block_exclusive_scan(s, &total);
@@ -416,7 +436,7 @@ __global__ void __launch_bounds__(kScanThreads) k_offsets_scan_tiles(unsigned lo
     }
 }
 
-template <bool BLOCKS>
+template <uint32_t PER>
 __global__ void __launch_bounds__(kScanThreads) k_offsets_apply(const uint32_t* counts, uint64_t n,
                                                                   const unsigned long long* tile_offs,
                                                                   unsigned long long* out_offs) {
@@ -427,7 +447,7 @@ __global__ void __launch_bounds__(kScanThreads) k_offsets_apply(const uint32_t* 
 #pragma unroll
     for (int k = 0; k < kScanPerThread; ++k) {
         const uint64_t i = first + k;
-        c[k] = i < n ? scan_term<BLOCKS>(counts[i]) : 0;
+        c[k] = i < n ? scan_term<PER>(counts[i]) : 0;
         s += c[k];
     }
     unsigned long long total;
@@ -503,6 +523,69 @@ __global__ void __launch_bounds__(256) k_gather(const uint32_t* pool, const Scan
             uint32_t* dst = out_words + (item_offs[item[u]] + first) * 3ull;
             if (lane < nw) dst[lane] = w0[u];
             if (lane + 32 < nw) dst[lane + 32] = w1[u];
+        }
+    }
+}
+
+// Placement of event blocks (StdMachine3's matches path): k_gather's walk, contract and arguments, but every event
+// is expanded here -- output_pos of its slot, the head record, for find_overlapping the whole parent chain.  The
+// scan loop stays free of these dependent loads; here they overlap across U blocks per warp and many warps.
+// Lane j of a warp takes event j of a block: a warp scan of the list lengths gives its place behind the block's
+// first match (header word 2), and the lane writes its list as consecutive 12-byte tuples.
+template <bool OVERLAP, int U>
+__global__ void __launch_bounds__(256) k_expand(const uint32_t* pool, const ScanCtrl* ctrl, uint32_t pool_blocks,
+                                                 const uint32_t* ev_counts, const unsigned long long* item_offs,
+                                                 uint64_t n_items, unsigned long long out_cap, const unsigned long long* base,
+                                                 uint32_t* out_words, const uint32_t* blkmap, const unsigned long long* pad_like,
+                                                 const uint4* outputs, const uint32_t* opos_tab) {
+    if (ctrl->overflow) return;
+    const unsigned long long b0m = base ? *base : 0ull;
+    if (b0m + item_offs[n_items] > out_cap) return;
+    out_words += b0m * 3ull;
+    if (pad_like) out_words += (*pad_like * 3ull) & 3ull;  // staged copy for k_push (k_gather)
+    const uint32_t used = min(ctrl->blk_cursor, pool_blocks);
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t warp = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const uint64_t n_warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t b0 = warp * U; b0 < used; b0 += n_warps * U) {
+        uint4 h[U], o[U];
+        uint2 ev[U];
+        uint32_t len[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const uint64_t b = b0 + u < used ? b0 + u : b0;
+            const uint32_t* blk = pool + (blkmap ? (uint64_t)blkmap[b] : b) * BLK_WORDS;
+            h[u] = *reinterpret_cast<const uint4*>(blk);  // {item, seq, first, -}
+            ev[u] = lane < BLK_EVENTS ? reinterpret_cast<const uint2*>(blk + BLK_HDR_WORDS)[lane] : make_uint2(0u, 0u);
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const uint32_t nev = min(BLK_EVENTS, ev_counts[h[u].x] - h[u].y * BLK_EVENTS);
+            const bool on = b0 + u < used && lane < nev;
+            const uint32_t op = on ? ld_u32(opos_tab + (ev[u].y & QSLOT_MASK)) : 0u;
+            o[u] = on ? ld_u4(outputs + (op - 1)) : make_uint4(0u, 0u, 0u, 0u);
+            len[u] = on ? (OVERLAP ? o[u].w : 1u) : 0u;
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            uint32_t inc = len[u];
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t t = __shfl_up_sync(0xffffffffu, inc, d);
+                if (lane >= (uint32_t)d) inc += t;
+            }
+            if (!len[u]) continue;
+            uint32_t* dst = out_words + (item_offs[h[u].x] + h[u].z + (inc - len[u])) * 3ull;
+            const uint32_t end = ev[u].x;
+            uint4 r = o[u];
+            for (uint32_t k = 0;;) {
+                dst[0] = end - r.y;
+                dst[1] = end;
+                dst[2] = r.x;
+                if (++k == len[u]) break;
+                dst += 3;
+                r = ld_u4(outputs + (r.z - 1));
+            }
         }
     }
 }
@@ -820,7 +903,7 @@ struct HostPinned {
 // different streams: enqueue_scan (items, scan kernel, offsets, block index) and enqueue_place (gather into the
 // caller's -- possibly peer-mapped -- buffers); finish_scan waits for the second and reports.
 struct Workspace {
-    DevBuf counts, tiles, ctrl, pool;
+    DevBuf counts, ev_counts, tiles, ctrl, pool;  // ev_counts: events per item (event blocks)
     DevBuf nseg, seg_first, item_hay, item_beg, item_offs, n_items_dev;  // segment table, per-item offsets
     DevBuf blk_first, blkmap, tiles2;  // pool blocks in output order (k_blk_index)
     DevBuf stage;  // shard groups: the job's dense matches, pushed to the gathering rank by k_push
@@ -835,6 +918,8 @@ struct Workspace {
     uint32_t job_pool_blocks = 0;
     uint64_t job_cap = 0;
     bool job_seg = false, job_ordered = false, job_open = false, job_placed = false;
+    bool job_events = false;
+    int job_mode = 0;  // the pool holds event blocks (StdMachine3): k_expand places them, not k_gather
     cudaStream_t job_stream = nullptr;
     // host-batch slices only: device staging and the slice's stream
     DevBuf text, offs, out, out_offs;
@@ -855,7 +940,7 @@ struct Workspace {
         return true;
     }
     void release() {
-        for (DevBuf* b : {&counts, &tiles, &ctrl, &pool, &text, &offs, &out, &out_offs, &nseg, &seg_first, &item_hay, &item_beg,
+        for (DevBuf* b : {&counts, &ev_counts, &tiles, &ctrl, &pool, &text, &offs, &out, &out_offs, &nseg, &seg_first, &item_hay, &item_beg,
                           &item_offs, &n_items_dev, &blk_first, &blkmap, &tiles2, &stage, &items_rk, &total_rk, &slot_hist, &rec_hist,
                           &hist_acc})
             if (b->p) {
@@ -1249,9 +1334,9 @@ void enqueue_seg_table(dach_dev* d, Workspace& W, const uint64_t* d_offs, uint64
     const uint64_t nt = (n + kScanTile - 1) / kScanTile;
     uint32_t* nseg = static_cast<uint32_t*>(W.nseg.p);
     k_seg_count<<<hb, 256, 0, st>>>(d_offs, n, seg_len, seg_from, nseg, P.ctrl);
-    k_offsets_tile_sums<false><<<(unsigned)nt, kScanThreads, 0, st>>>(nseg, n, tiles);
+    k_offsets_tile_sums<1><<<(unsigned)nt, kScanThreads, 0, st>>>(nseg, n, tiles);
     k_offsets_scan_tiles<<<1, kScanThreads, 0, st>>>(tiles, nt);
-    k_offsets_apply<false><<<(unsigned)nt, kScanThreads, 0, st>>>(nseg, n, tiles, seg_first);
+    k_offsets_apply<1><<<(unsigned)nt, kScanThreads, 0, st>>>(nseg, n, tiles, seg_first);
     k_seg_fill<<<hb1, 256, 0, st>>>(seg_first, nseg, n, seg_len, static_cast<uint32_t*>(W.item_hay.p),
                                     static_cast<uint32_t*>(W.item_beg.p), static_cast<unsigned long long*>(W.n_items_dev.p));
     d->launches += 5;
@@ -1281,6 +1366,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     W.job_items = n;
     W.job_seg = false;
     W.job_ordered = false;
+    W.job_events = false;
     W.job_stream = st;
     W.job_open = true;
     if (!ensure(W.ctrl, sizeof(ScanCtrl)) || !ensure(W.item_offs, 16)) return DACH_CUDA_ERROR;
@@ -1307,6 +1393,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     const bool std2 = v1 && !d->charwise && mode != M_LEFTMOST && d->opt_kernel >= 2 && d->root_base != 0;
     const bool std3 = std2 && d->opt_kernel >= 3;
     const bool duo = std3 && d->opt_kernel >= 4 && ctas_per_sm == 1;
+    const bool events = std3 && !duo;  // StdMachine3's matches path stores events (k_scan_machine)
 
     if (d_state_io && !std2 && !cw_machine) {
         set_error("stream chunks need a Standard lane machine (find / find_overlapping, at most 2^24 states, bytewise: "
@@ -1357,7 +1444,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     if (pool_blocks64 > 0xffffff00ull) pool_blocks64 = 0xffffff00ull;
     const uint32_t pool_blocks = (uint32_t)pool_blocks64;
     if (!ensure(W.counts, n_items_max * 4) || !ensure(W.tiles, n_tiles * 8) || !ensure(W.item_offs, (n_items_max + 1) * 8) ||
-        !ensure(W.pool, (size_t)pool_blocks * BLK_WORDS * 4))
+        !ensure(W.pool, (size_t)pool_blocks * BLK_WORDS * 4) || (events && !ensure(W.ev_counts, n_items_max * 4)))
         return DACH_CUDA_ERROR;
     if (seg && (!ensure(W.nseg, n * 4) || !ensure(W.seg_first, (n + 1) * 8) || !ensure(W.item_hay, n_items_max * 4) ||
                 !ensure(W.item_beg, n_items_max * 4) || !ensure(W.n_items_dev, 8)))
@@ -1365,6 +1452,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
 
     ScanParams P = image_params(d, d_text, text_lo, text_end, d_offs, n);
     P.counts = static_cast<uint32_t*>(W.counts.p);
+    P.ev_counts = events ? static_cast<uint32_t*>(W.ev_counts.p) : nullptr;
     P.pool = static_cast<uint32_t*>(W.pool.p);
     P.pool_blocks = pool_blocks;
     P.ctrl = static_cast<ScanCtrl*>(W.ctrl.p);
@@ -1377,6 +1465,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     ++d->launches;
     if (seg) {
         cudaMemsetAsync(W.counts.p, 0, n_items_max * 4, st);  // items past the real count stay empty
+        if (events) cudaMemsetAsync(W.ev_counts.p, 0, n_items_max * 4, st);
         enqueue_seg_table(d, W, d_offs, n, seg_len, seg_from, P, st);
     }
     cudaEventRecord(W.ev[3], st);
@@ -1389,9 +1478,9 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
                  "k_scan launch"))
         return DACH_CUDA_ERROR;
     cudaEventRecord(W.ev[1], st);
-    k_offsets_tile_sums<false><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles);
+    k_offsets_tile_sums<1><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles);
     k_offsets_scan_tiles<<<1, kScanThreads, 0, st>>>(tiles, n_tiles);
-    k_offsets_apply<false><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles, item_offs);
+    k_offsets_apply<1><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles, item_offs);
     d->launches += 4;
     // batches whose match blocks stay in L2 anyway are copied in pool order (four launches fewer)
     const bool ordered = d->opt_gather_ordered >= 2 || (d->opt_gather_ordered == 1 && text_bytes >= (256ull << 20));
@@ -1400,9 +1489,15 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
             return DACH_CUDA_ERROR;
         unsigned long long* tiles2 = static_cast<unsigned long long*>(W.tiles2.p);
         unsigned long long* blk_first = static_cast<unsigned long long*>(W.blk_first.p);
-        k_offsets_tile_sums<true><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles2);
-        k_offsets_scan_tiles<<<1, kScanThreads, 0, st>>>(tiles2, n_tiles);
-        k_offsets_apply<true><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles2, blk_first);
+        if (events) {  // blocks per item: ceil(events / BLK_EVENTS)
+            k_offsets_tile_sums<BLK_EVENTS><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.ev_counts, n_items_max, tiles2);
+            k_offsets_scan_tiles<<<1, kScanThreads, 0, st>>>(tiles2, n_tiles);
+            k_offsets_apply<BLK_EVENTS><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.ev_counts, n_items_max, tiles2, blk_first);
+        } else {
+            k_offsets_tile_sums<BLK_MATCHES><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles2);
+            k_offsets_scan_tiles<<<1, kScanThreads, 0, st>>>(tiles2, n_tiles);
+            k_offsets_apply<BLK_MATCHES><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles2, blk_first);
+        }
         k_blk_index<<<d->sm_count * 8, 256, 0, st>>>(P.pool, P.ctrl, pool_blocks, blk_first, static_cast<uint32_t*>(W.blkmap.p));
         d->launches += 4;
     }
@@ -1411,6 +1506,8 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     W.job_items = n_items_max;
     W.job_seg = seg;
     W.job_ordered = ordered;
+    W.job_events = events;
+    W.job_mode = mode;
     W.job_pool_blocks = pool_blocks;
     return DACH_OK;
 }
@@ -1445,7 +1542,15 @@ int enqueue_place(dach_dev* d, Workspace& W, dach_match* d_out, uint64_t out_cap
             g_cap = W.job_cap;
         }
         const unsigned long long* pad_like = staged ? d_base : nullptr;
-        if (d->opt_gather_u >= 8)
+        if (W.job_events) {
+            const uint32_t* ev_counts = static_cast<const uint32_t*>(W.ev_counts.p);
+            if (W.job_mode == M_OVERLAPPING)
+                k_expand<true, 2><<<gather_grid, 256, 0, st>>>(pool, ctrl, W.job_pool_blocks, ev_counts, item_offs, n_items, g_cap, g_base,
+                                                                out_words, blkmap, pad_like, d->d_outputs, d->d_opos);
+            else
+                k_expand<false, 2><<<gather_grid, 256, 0, st>>>(pool, ctrl, W.job_pool_blocks, ev_counts, item_offs, n_items, g_cap, g_base,
+                                                                 out_words, blkmap, pad_like, d->d_outputs, d->d_opos);
+        } else if (d->opt_gather_u >= 8)
             k_gather<8><<<gather_grid, 256, 0, st>>>(pool, ctrl, W.job_pool_blocks, counts, item_offs, n_items, g_cap, g_base, out_words, blkmap, pad_like);
         else if (d->opt_gather_u <= 2)
             k_gather<2><<<gather_grid, 256, 0, st>>>(pool, ctrl, W.job_pool_blocks, counts, item_offs, n_items, g_cap, g_base, out_words, blkmap, pad_like);

@@ -18,6 +18,8 @@
 //                  that k_scan_duo can keep two fetches in flight; serves stream chunks
 //   - SinkOps      COUNT / FIRST / HIST on StdMachine3, LmMachine, CwMachine: their drain() / begin_item() for
 //                  the other result kinds (sinks: Emitter, CountSink, FirstSink, HistSink)
+//   - EventOps     the matches path of StdMachine3: events stored into event blocks (EventSink), expanded after
+//                  the scan by k_expand
 //
 // Device image (built by dev_image.cpp from the validated host automaton):
 //   wide bytewise record  uint4 {base, efail, fbase, opos<<8 | check}      16 B / slot
@@ -92,6 +94,15 @@ constexpr int M_FIND = 0, M_OVERLAPPING = 1, M_NO_SUFFIX = 2, M_LEFTMOST = 3;
 constexpr uint32_t BLK_WORDS = 64;
 constexpr uint32_t BLK_MATCHES = 15;
 constexpr uint32_t BLK_SLOT_WORDS = 4;
+// Event blocks (matches path of StdMachine3): the same 256 bytes, header {item, seq, first, -} -- `first` is the
+// item-relative index of the block's first match -- then 30 events {end, packed slot} of 8 bytes.  k_expand turns
+// them into tuples; the per-item event count (ScanParams::ev_counts) says how many events a block holds.
+constexpr uint32_t BLK_EVENTS = 30;
+constexpr uint32_t BLK_HDR_WORDS = 4;
+// Queue entries of StdMachine3 carry the state's output-list length in the slot's high byte (compact slots are
+// < 2^24), saturated at QLEN_ESCAPE: that value means "255 or more, read the head record's chain word".
+constexpr uint32_t QSLOT_MASK = 0xffffffu;
+constexpr uint32_t QLEN_ESCAPE = 255u;
 
 struct ScanCtrl {
     unsigned long long next_item;  // dynamic work counter
@@ -134,7 +145,8 @@ struct ScanParams {
                          // written at its end; nullptr for ordinary scans (every haystack starts in ROOT)
     uint32_t seg_from;  // haystacks below this index stay whole (one item each): only the tail of a batch is cut
     // results
-    uint32_t* counts;  // matches per item
+    uint32_t* counts;     // matches per item
+    uint32_t* ev_counts;  // event blocks: events stored per item
     uint32_t* pool;
     uint32_t pool_blocks;
     ScanCtrl* ctrl;
@@ -193,6 +205,13 @@ DACH_HD void st_stream_u4(uint32_t* p, uint32_t a, uint32_t b, uint32_t c, uint3
                  : "memory");
 #else
     p[0] = a, p[1] = b, p[2] = c, p[3] = d;
+#endif
+}
+DACH_HD void st_stream_u2(uint32_t* p, uint32_t a, uint32_t b) {
+#if defined(__CUDA_ARCH__)
+    asm volatile("st.global.L2::cache_hint.v2.u32 [%0], {%1,%2}, %3;" ::"l"(p), "r"(a), "r"(b), "l"(c_l2pol[2]) : "memory");
+#else
+    p[0] = a, p[1] = b;
 #endif
 }
 
@@ -340,6 +359,45 @@ struct FirstSink {
 DACH_HD uint32_t chain_len(const ScanParams& P, uint32_t opos) {
     return ld_u32(reinterpret_cast<const uint32_t*>(P.outputs + (opos - 1)) + 3);
 }
+// the list length a StdMachine3 queue entry carries; the escape value costs the two loads it saves otherwise
+DACH_HD uint32_t qentry_len(const ScanParams& P, const uint32_t* opos_tab, uint32_t packed) {
+    const uint32_t b = packed >> 24;
+    return b != QLEN_ESCAPE ? b : chain_len(P, ld_u32(opos_tab + (packed & QSLOT_MASK)));
+}
+
+// Matches path of StdMachine3: events go to event blocks as they are, k_expand expands them after the scan.
+// Blocks are taken in the warp-converged service phase with one warp-aggregated atomic (EventOps::drain).
+struct EventSink {
+    static constexpr int KIND = RK_MATCHES;
+    uint32_t* blk;   // current block (nullptr: none yet, or the pool is exhausted)
+    uint32_t fill;   // events in the current block; BLK_EVENTS when the next event needs a new block
+    uint32_t nev;    // events of the current item
+    uint32_t count;  // matches of the current item
+    uint32_t item;
+    DACH_HD void begin(uint32_t item_id) {
+        blk = nullptr;
+        fill = BLK_EVENTS;
+        nev = 0;
+        count = 0;
+        item = item_id;
+    }
+    // block `b` of the pool becomes current; its first event is match `count` of the item
+    DACH_HD void open(const ScanParams& P, uint32_t b) {
+        if (b < P.pool_blocks) {
+            blk = P.pool + (size_t)b * BLK_WORDS;
+            st_stream_u4(blk, item, nev / BLK_EVENTS, count, 0u);
+        } else {
+            blk = nullptr;
+            P.ctrl->overflow = 1u;
+        }
+        fill = 0;
+    }
+    DACH_HD void finish(const ScanParams& P) {
+        P.counts[item] = count;
+        P.ev_counts[item] = nev;
+    }
+    DACH_HD bool stopped() const { return false; }
+};
 
 // Walk a merged output list from `opos` (1-based, 0 = end), emitting every pattern ending
 // at `end` (src/bytewise/iter.rs:134-148).
@@ -727,7 +785,8 @@ DACH_HD void scan_leftmost(const ScanParams& P, const RecView& V, TextWin& T, SI
 //     w0 = BASE << 8 | CHECK                      src/bytewise.rs:1131-1137
 //     w1 = efail << 8 | flags                     flags: CF_OUT (state has an output list),
 //                                                        CF_F2ROOT (efail(efail) == ROOT)
-//     w2 = fbase << 8                             BASE of efail
+//     w2 = fbase << 8 | min(list length, 255)     BASE of efail; the length of the state's output list (0: none),
+//                                                 queued with StdMachine3's find_overlapping events.  Readers shift.
 //     w3 = child signature: bit (c & 31) is set iff the state has a child labelled c
 // The signature answers "no child for this byte" without touching the child slot: on the C3
 // workload 0.31 of the 1.28 probes per byte were misses of the state's own children; with it
@@ -773,7 +832,7 @@ struct LaneStd {
     uint32_t cb;   // BASE (0: no children)
     uint32_t sig;  // child signature
     uint32_t nf;   // raw word 1: efail << 8 | CF_* flags
-    uint32_t nfb;  // raw word 2: fbase << 8
+    uint32_t nfb;  // raw word 2: fbase << 8 | list length
     uint32_t addr; // slot being fetched; after a landing: the slot landed on
     uint32_t qn;   // queued events
     uint32_t fl;   // F_* flags
@@ -839,6 +898,7 @@ struct StdMachine {
     static constexpr bool LAZY = false;
     static constexpr bool LEAN = false;
     static constexpr uint32_t IDLE = 0;
+    static constexpr bool QLEN = false;
     static DACH_HD void finish_item(const LaneStd&, const ScanParams&) {}
     static DACH_HD const uint8_t* block_of(const LaneStd& L) {
         return reinterpret_cast<const uint8_t*>(((uintptr_t)L.hay + L.pos) & ~(uintptr_t)15);
@@ -1072,6 +1132,7 @@ struct LmMachine {
     static constexpr bool LAZY = true;
     static constexpr bool LEAN = false;
     static constexpr uint32_t IDLE = 0;
+    static constexpr bool QLEN = false;
     static DACH_HD void finish_item(const LaneLm&, const ScanParams&) {}
     using Std = StdMachine<M_LEFTMOST>;
 
@@ -1311,6 +1372,7 @@ struct CwMachine {
     static constexpr bool LAZY = true;
     static constexpr bool LEAN = false;
     static constexpr uint32_t IDLE = 0;
+    static constexpr bool QLEN = false;
     // the item is complete: hand the state on to the next chunk of the stream (the charwise steppers,
     // src/charwise/iter.rs:403-534; the charwise image keeps the crate's state ids)
     static DACH_HD void finish_item(const LaneCw& L, const ScanParams& P) {
@@ -1661,6 +1723,7 @@ struct StdMachine2 {
     static constexpr bool LAZY = true;
     static constexpr bool LEAN = false;
     static constexpr uint32_t IDLE = 0;
+    static constexpr bool QLEN = false;
 
     static DACH_HD const uint8_t* block_of(const Lane2& L) {
         return reinterpret_cast<const uint8_t*>(((uintptr_t)L.hay + L.pos) & ~(uintptr_t)7);
@@ -1905,6 +1968,8 @@ struct StdMachine3 {
     static constexpr bool LAZY = true;
     static constexpr bool LEAN = true;
     static constexpr uint32_t IDLE = F3_STOP;
+    static constexpr bool QLEN = true;  // find_overlapping entries carry the list length (QSLOT_MASK)
+    static constexpr int ITER = MODE;
 
     // one record: the hot region's leading slots from shared memory, everything else through L1 / L2
     static DACH_HD uint4 fetch(const StdEnv& Ev, uint32_t a) {
@@ -1960,9 +2025,9 @@ struct StdMachine3 {
         if (L.ap == L.ap_end) L.fl |= F_DONE | F3_STOP;
         if (L.nf & CF_OUT) {
             DACH_STAT(pushes);
-            QEntry e;  // one 8-byte store: (end, slot); output_pos is looked up when the queue is drained
+            QEntry e;  // one 8-byte store: (end, slot | list length << 24); output_pos is looked up after the scan
             e.end = L.ap - L.hay_lo;
-            e.opos = L.addr;
+            e.opos = MODE == M_OVERLAPPING ? L.addr | (L.r2 << 24) : L.addr;  // the length: low byte of record word 2
             Ev.q[L.qn * Ev.q_stride] = e;
             if (++L.qn == (uint32_t)LANE_Q) L.fl |= F3_STOP;
             if (MODE == M_FIND) to_root(L, Ev);  // every next() restarts at ROOT (src/bytewise/iter.rs:87)
@@ -2037,7 +2102,7 @@ struct StdMachine3 {
             if (j < L.qn) {
                 const QEntry e = Ev.q[j * Ev.q_stride];
                 if (e.end >= L.from) {  // a segment reports only what ends inside it
-                    const uint32_t opos = ld_u32(Ev.opos + e.opos);  // the entry holds the slot
+                    const uint32_t opos = ld_u32(Ev.opos + (e.opos & QSLOT_MASK));  // the entry holds the slot
                     if (MODE == M_OVERLAPPING)
                         emit_chain(P, E, opos, e.end);
                     else
@@ -2109,7 +2174,7 @@ struct StdMachine3 {
         if (MODE != M_FIND && (Ev.root_flags & CF_OUT) && beg == 0) {
             QEntry e;  // the iterator starts in ROOT with ROOT's output list pending at position 0
             e.end = 0;
-            e.opos = D_ROOT;
+            e.opos = MODE == M_OVERLAPPING ? D_ROOT | (Ev.root_rec.z << 24) : D_ROOT;
             Ev.q[0] = e;
             L.qn = 1;
         }
@@ -2145,7 +2210,7 @@ struct SinkOps {
         E.begin((uint32_t)item);
         if constexpr (RK == RK_FIRST) {
             if (L.qn) {  // ROOT's list at position 0 (an empty pattern): reportable at once
-                E.emit(P, 0, 0, ld_u4(P.outputs + (ld_u32(Ev.opos + Ev.q[0].opos) - 1)).x);
+                E.emit(P, 0, 0, ld_u4(P.outputs + (ld_u32(Ev.opos + (Ev.q[0].opos & QSLOT_MASK)) - 1)).x);
                 L.qn = 0;
                 L.fl |= F_DONE | M::IDLE;
             } else {
@@ -2160,7 +2225,10 @@ struct SinkOps {
             for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j) {
                 if (j < L.qn) {
                     const QEntry e = Ev.q[j * Ev.q_stride];
-                    if (e.end >= L.from) E.count += MODE == M_OVERLAPPING ? chain_len(P, ld_u32(Ev.opos + e.opos)) : 1u;
+                    if (e.end >= L.from)
+                        E.count += MODE != M_OVERLAPPING ? 1u
+                                   : M::QLEN         ? qentry_len(P, Ev.opos, e.opos)
+                                                     : chain_len(P, ld_u32(Ev.opos + e.opos));
                 }
             }
             L.qn = 0;
@@ -2168,7 +2236,7 @@ struct SinkOps {
             for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j) {
                 if (j < L.qn) {
                     const QEntry e = Ev.q[j * Ev.q_stride];
-                    if (e.end >= L.from) E.event(P, e.opos);  // the entry holds the slot
+                    if (e.end >= L.from) E.event(P, e.opos & QSLOT_MASK);  // the entry holds the slot
                 }
             }
             L.qn = 0;
@@ -2176,13 +2244,62 @@ struct SinkOps {
             if (L.qn == (uint32_t)LANE_Q) {
                 const QEntry e = Ev.q[(LANE_Q - 1) * Ev.q_stride];
                 if (e.end >= L.from) {
-                    emit_head(P, E, ld_u32(Ev.opos + e.opos), e.end);
+                    emit_head(P, E, ld_u32(Ev.opos + (e.opos & QSLOT_MASK)), e.end);
                     L.fl |= F_DONE | M::IDLE;
                 }
             }
             if (!(L.fl & F_DONE)) L.qn = (uint32_t)LANE_Q - 1;
         }
         if (!(L.fl & F_DONE)) L.fl &= ~M::IDLE;
+    }
+};
+
+// =============================================================================================
+// The matches path of StdMachine3: the drain stores events, k_expand (dev_scan.cu) expands them.
+//
+// The drain does no dependent load: each reportable entry (end >= L.from) is one 8-byte store into the lane's
+// current event block, and the item's match count grows by the list length the entry carries (1 for find /
+// no_suffix, whose events report the list's head only).  A lane stores at most LANE_Q < BLK_EVENTS events per
+// service phase, so it needs at most one new block per phase; the kernel hands those out with one warp-aggregated
+// atomic between need_block() and drain().
+// =============================================================================================
+template <int MODE>
+struct EventOps {
+    using M = StdMachine3<MODE>;
+
+    static DACH_HD void begin_item(Lane3& L, const ScanParams& P, const StdEnv& Ev, EventSink& E, uint64_t item,
+                                   const uint8_t* emu_lo) {
+        Emitter unused;  // the machine only names the item to its sink
+        M::begin_item(L, P, Ev, unused, item, emu_lo);
+        E.begin((uint32_t)item);
+    }
+
+    static DACH_HD uint32_t reportable(const Lane3& L, const StdEnv& Ev) {
+        uint32_t n = 0;
+        for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j)
+            if (j < L.qn && Ev.q[j * Ev.q_stride].end >= L.from) ++n;
+        return n;
+    }
+    static DACH_HD bool need_block(const Lane3& L, const StdEnv& Ev, const EventSink& E) {
+        return reportable(L, Ev) > BLK_EVENTS - E.fill;
+    }
+
+    // blk: the pool block this lane was given this phase (used only if need_block() said so)
+    static DACH_HD void drain(Lane3& L, const StdEnv& Ev, const ScanParams& P, EventSink& E, uint32_t blk) {
+        for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j) {
+            if (j < L.qn) {
+                const QEntry e = Ev.q[j * Ev.q_stride];
+                if (e.end >= L.from) {  // a segment reports only what ends inside it
+                    if (E.fill == BLK_EVENTS) E.open(P, blk);
+                    if (E.blk) st_stream_u2(E.blk + BLK_HDR_WORDS + 2 * E.fill, e.end, e.opos);
+                    ++E.fill;
+                    ++E.nev;
+                    E.count += MODE == M_OVERLAPPING ? qentry_len(P, Ev.opos, e.opos) : 1u;
+                }
+            }
+        }
+        L.qn = 0;
+        if (!(L.fl & F_DONE)) L.fl &= ~F3_STOP;
     }
 };
 

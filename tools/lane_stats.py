@@ -7,7 +7,14 @@ No GPU needed.  Usage: python tools/lane_stats.py [C2|C3|C5 ...]
 
 reports instead how the lane machines' output events (what a HIST scan counts per state) spread over the compact
 slots: the share on the 1 / 64 / 1024 / 4096 busiest slots and on the leading 1024 / 4096 slots (what option hist_smem
-counts in shared memory), from tests/emu_hist."""
+counts in shared memory), from tests/emu_hist.
+
+    python tools/lane_stats.py --lists [C3 C2 ...]
+
+reports the output-list lengths of find_overlapping events (the matches that end at one position of a haystack come
+from one event, and there are as many as the landed state's list is long): their distribution, and the share of
+events whose list is too long for the length byte StdMachine3 queues with an event (255 or more: the drain reads the
+head record's chain word instead), from the oracle's matches."""
 import ctypes as C
 import os
 import sys
@@ -79,8 +86,31 @@ def event_shares(name, n_hay=256):
     print("   leading slots:  " + "  ".join("< %d %.1f %%" % (k, 100.0 * lead[k] / max(all_, 1)) for k in tops[2:]))
 
 
+def list_lengths(name, n_hay=256):
+    cfg = S.config(name)
+    ps = S.make_patterns(cfg)
+    pool, b = S.make_pool(cfg, ps, 16 << 20)
+    opma = O.OraclePma.build_packed(ps.blob, ps.offs)
+    hay_len = min(cfg["hay_len"], 1 << 14)
+    starts = S.window_starts(b, len(pool), n_hay, hay_len)
+    text, offs = S.materialise_host(pool, starts, hay_len)
+    ref = opma.scan_batch(O.FIND_OVERLAPPING, text, offs, want_matches=True)
+    hay = np.repeat(np.arange(n_hay, dtype=np.uint64), ref["counts"].astype(np.int64))
+    _, lens = np.unique((hay << np.uint64(32)) | ref["matches"]["end"].astype(np.uint64), return_counts=True)
+    n = max(len(lens), 1)
+    print("== %s find_overlapping: %d events, %.4f per byte, %.3f matches per event, longest list %d"
+          % (name, len(lens), len(lens) / len(text), lens.sum() / n, lens.max() if len(lens) else 0))
+    bins = [(1, 1), (2, 2), (3, 4), (5, 16), (17, 254), (255, 1 << 62)]
+    print("   list length:  " + "  ".join("%s %.2f %%" % (str(lo) if lo == hi else "%d+" % lo if hi > 1 << 40 else "%d-%d" % (lo, hi),
+                                                           100.0 * np.count_nonzero((lens >= lo) & (lens <= hi)) / n) for lo, hi in bins))
+    print("   events that take the escape (list >= 255): %.4f %%" % (100.0 * np.count_nonzero(lens >= 255) / n))
+
+
 if __name__ == "__main__":
-    if sys.argv[1:2] == ["--events"]:
+    if sys.argv[1:2] == ["--lists"]:
+        for nm in (sys.argv[2:] or ["C3", "C2"]):
+            list_lengths(nm)
+    elif sys.argv[1:2] == ["--events"]:
         for nm in (sys.argv[2:] or list(EVENT_CONFIGS)):
             event_shares(nm)
     else:

@@ -7,7 +7,7 @@ native, so this is a subset of tests/test_gpu_parity.py that still launches ever
 
 Golden vectors (all iterators x bytewise / charwise), random batches on every kernel option, text buffers at odd
 addresses and with no slack after the last byte (the 8-byte text loads must not touch anything outside), stream
-chunks, counts and first matches, per-pattern histograms (both keys, shared-memory counters on and off), asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
+chunks, event blocks with output lists of 255 and more (k_expand in pool and output order), counts and first matches, per-pattern histograms (both keys, shared-memory counters on and off), asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
 import json
 import os
 import sys
@@ -87,6 +87,28 @@ def random_batches():
                 m = r.matches.cpu().numpy().astype(np.uint32)
                 assert m.tobytes() == ref["matches"].tobytes(), ("odd address", cw, kind, mode)
                 n_scans += 1
+
+
+def event_blocks():
+    """StdMachine3's event blocks with lists too long for the length byte, placed by k_expand in pool order and in
+    output order, whole and in segments."""
+    global n_scans
+    pats = [b"a" * k for k in range(1, 301)] + [b"ba"]
+    hays = [b"a" * 400, b"xa" + b"a" * 260 + b"b" + b"a" * 300, b"", b"ba" * 40] * 8
+    offs = np.zeros(len(hays) + 1, dtype=np.uint64)
+    offs[1:] = np.cumsum([len(h) for h in hays])
+    text = np.frombuffer(b"".join(hays), dtype=np.uint8)
+    pma, opma = D.DoubleArrayAhoCorasick.new(pats), O.OraclePma.build(pats)
+    for mode in (D.FIND, D.FIND_OVERLAPPING, D.FIND_OVERLAPPING_NO_SUFFIX):
+        ref = opma.scan_batch(ORC[mode], text, offs, want_matches=True)
+        for opts in ({"gather_ordered": 0}, {"gather_ordered": 2}, {"gather_ordered": 2, "seg_len": 64}):
+            for k, v in opts.items():
+                pma.set_option(k, v)
+            r = pma.scan_batch_host(mode, text, offs)
+            assert r.matches.tobytes() == ref["matches"].tobytes(), (mode, opts)
+            n_scans += 1
+            pma.set_option("seg_len", 0)
+        pma.set_option("gather_ordered", 1)
 
 
 def counts_and_first():
@@ -211,6 +233,7 @@ def streams_jobs_groups():
 if __name__ == "__main__":
     golden()
     random_batches()
+    event_blocks()
     counts_and_first()
     histograms()
     streams_jobs_groups()
