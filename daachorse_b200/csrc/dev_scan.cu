@@ -700,12 +700,14 @@ __device__ __forceinline__ unsigned long long global_ns() {
 }
 constexpr unsigned long long kGroupTimeoutNs = 20ull * 1000 * 1000 * 1000;  // a peer that never arrives must not hang the GPU
 
-// this rank's match count of the step goes to every rank's control block
-__global__ void k_group_publish(GroupPeers peers, int world, int rank, unsigned long long step, const unsigned long long* total) {
+// this rank's match count of the step goes to every rank's control block (exact past 2^32 matches per haystack:
+// the carries of the per-item counts are added back, finish_scan)
+__global__ void k_group_publish(GroupPeers peers, int world, int rank, unsigned long long step, const unsigned long long* total,
+                                const ScanCtrl* ctrl) {
     const int j = threadIdx.x;
     if (j >= world) return;
     GroupCtl* c = peers.ctl[j];
-    c->total[step & 1][rank] = *total;
+    c->total[step & 1][rank] = *total + ((unsigned long long)ctrl->carries << 32);
     __threadfence_system();
     st_release_sys(&c->total_seq[step & 1][rank], step);
 }
@@ -919,6 +921,7 @@ struct Workspace {
     uint64_t job_cap = 0;
     bool job_seg = false, job_ordered = false, job_open = false, job_placed = false;
     bool job_events = false;
+    bool refused = false;  // finish_scan: a haystack passed 2^32 matches (*needed exact, status DACH_INVALID_ARGUMENT)
     int job_mode = 0;  // the pool holds event blocks (StdMachine3): k_expand places them, not k_gather
     cudaStream_t job_stream = nullptr;
     // host-batch slices only: device staging and the slice's stream
@@ -1033,6 +1036,9 @@ struct dach_dev {
     cudaEvent_t ev_ref = nullptr;  // time zero of dach_job_times (recorded at the first job scan)
     double last_scan_ms = 0, last_total_ms = 0;
     uint64_t last_h2d = 0, last_d2h = 0;
+    // the handle's owner plus one per live job: dach_dev_free may come before the jobs are freed (a garbage collector
+    // finalises in any order), and the jobs still read the image and d->device until then
+    std::atomic<int> refs{1};
 };
 
 // one asynchronous scan with its own workspace (dach_job_*)
@@ -1050,6 +1056,7 @@ struct DeviceGuard {
     explicit DeviceGuard(int dev) {
         if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
         ok = cuda_ok(cudaSetDevice(dev), "cudaSetDevice");
+        if (!ok) cudaGetLastError();  // reported here; it must not resurface as the error of a later, unrelated launch
     }
     ~DeviceGuard() {
         if (prev >= 0) cudaSetDevice(prev);
@@ -1354,6 +1361,7 @@ void enqueue_seg_table(dach_dev* d, Workspace& W, const uint64_t* d_offs, uint64
 int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
                  uint64_t text_bytes, const uint64_t* d_offs, uint64_t n, uint64_t cap_matches, cudaStream_t st,
                  uint32_t* d_state_io = nullptr) {
+    W.refused = false;
     if (n > 0xfffffff0ull) {
         set_error("too many haystacks in one batch (max 2^32-16)");
         return DACH_INVALID_ARGUMENT;
@@ -1592,14 +1600,25 @@ int enqueue_place(dach_dev* d, Workspace& W, dach_match* d_out, uint64_t out_cap
 
 // ---- wait for the placement, report ----------------------------------------------------------------------
 int finish_scan(dach_dev* d, Workspace& W, uint64_t out_cap, uint64_t* needed) {
+    W.refused = false;
     if (!cuda_ok(cudaEventSynchronize(W.ev_placed), "scan pipeline")) return DACH_CUDA_ERROR;
     float ms = 0;
     if (cudaEventElapsedTime(&ms, W.ev[3], W.ev[1]) == cudaSuccess) d->last_scan_ms = ms;
     if (cudaEventElapsedTime(&ms, W.ev[0], W.ev[2]) == cudaSuccess) d->last_total_ms = ms;
-    const uint64_t total = W.pinned->total;
+    // every carry of a per-item u32 count is 2^32 matches item_offs[n] does not hold (count_carry, scan_lane.cuh)
+    const uint64_t total = W.pinned->total + ((uint64_t)W.pinned->ctrl.carries << 32);
     if (needed) *needed = total;
     if (W.pinned->ctrl.bad_offsets) {
         set_error("haystack offsets must be ascending and inside text_bytes, and no haystack may reach 4 GiB (match positions are u32)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    if (W.pinned->ctrl.carries) {
+        // no capacity helps: the match list of one haystack is indexed in 32 bits
+        W.refused = true;
+        char buf[256];
+        snprintf(buf, sizeof(buf), "a haystack yields 2^32 or more matches (batch total %llu): its match list cannot be placed; "
+                 "count it with dach_dev_count_batch / dach_dev_hist_batch instead", (unsigned long long)total);
+        set_error(buf);
         return DACH_INVALID_ARGUMENT;
     }
     if (W.pinned->ctrl.overflow || total > out_cap) {
@@ -1759,7 +1778,7 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
     for (Workspace& w : d->slot)
         if (!w.init(true)) return DACH_CUDA_ERROR;
     // every slot's previous work must be finished before its buffers are reused
-    bool overflow = false;
+    bool overflow = false, refused = false;
     uint64_t base = 0;
     const bool trace = getenv("DACH_DEBUG") != nullptr;
     double t_reuse = 0, t_scan = 0, t_final = 0, gpu_ms = 0;
@@ -1798,8 +1817,10 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
         }
         t_scan += now() - t_s0;
         gpu_ms += d->last_total_ms;
-        if (rc != DACH_OK && rc != DACH_OUTPUT_OVERFLOW) return rc;
-        if (base + s.total > out_cap) overflow = true;
+        // a haystack past 2^32 matches: nothing is copied back, the other slices are still counted for *needed
+        if (rc == DACH_INVALID_ARGUMENT && W.refused) refused = true;
+        else if (rc != DACH_OK && rc != DACH_OUTPUT_OVERFLOW) return rc;
+        if (refused || base + s.total > out_cap) overflow = true;
         if (!overflow) {
             // the slice's final offset is the next slice's first one: only the last slice copies it
             const uint64_t no = (k + 1 == slices.size()) ? ns + 1 : ns;
@@ -1819,6 +1840,13 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
         fprintf(stderr, "dach_scan_batch_host: %zu slices, %.2f ms total: waiting for slot reuse %.2f, in scan_locked %.2f, final D2H wait %.2f; kernels %.2f ms\n",
                 slices.size(), now() - t_begin, t_reuse, t_scan, t_final, gpu_ms);
     if (needed) *needed = base;
+    if (refused) {
+        char buf[256];
+        snprintf(buf, sizeof(buf), "a haystack yields 2^32 or more matches (batch total %llu): its match list cannot be placed; "
+                 "count it with dach_count_batch_host / dach_hist_batch_host instead", (unsigned long long)base);
+        set_error(buf);
+        return DACH_INVALID_ARGUMENT;
+    }
     if (overflow) {
         set_error("output capacity too small");
         return DACH_OUTPUT_OVERFLOW;
@@ -2209,7 +2237,7 @@ int dach_dev_upload(const dach_pma* pma, int device, dach_dev** out) {
 }
 
 void dach_dev_free(dach_dev* d) {
-    if (!d) return;
+    if (!d || --d->refs > 0) return;  // jobs of this device are still alive: the last dach_job_free releases it
     DeviceGuard g(d->device);
     cudaFree(d->image_base);
     if (d->ev_ref) cudaEventDestroy(d->ev_ref);
@@ -2349,6 +2377,7 @@ int dach_job_create(dach_dev* d, dach_job** out) {
             j->W.release();
             return DACH_CUDA_ERROR;
         }
+        ++d->refs;
         *out = j.release();
         return DACH_OK;
     });
@@ -2356,10 +2385,14 @@ int dach_job_create(dach_dev* d, dach_job** out) {
 
 void dach_job_free(dach_job* j) {
     if (!j) return;
-    DeviceGuard g(j->d->device);
-    if (j->W.job_open) cudaEventSynchronize(j->W.ev_placed);
-    j->W.release();
+    dach_dev* d = j->d;
+    {
+        DeviceGuard g(d->device);
+        if (j->W.job_open) cudaEventSynchronize(j->W.ev_placed);
+        j->W.release();
+    }
     delete j;
+    dach_dev_free(d);  // this job's reference (frees the device if its owner let go first)
 }
 
 int dach_job_scan(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
@@ -2598,7 +2631,7 @@ int dach_group_place(dach_group* G, dach_job* j, uint64_t hay_base, int last, vo
         // calling for step s says the result of step s-1 has been consumed: its buffers are free again
         if (G->rank == 0 && step > 1) k_group_release<<<1, kMaxRanks, 0, st>>>(G->peers, G->world, step - 1);
         const unsigned long long* total = static_cast<const unsigned long long*>(W.item_offs.p) + W.job_items;
-        k_group_publish<<<1, kMaxRanks, 0, st>>>(G->peers, G->world, G->rank, step, total);
+        k_group_publish<<<1, kMaxRanks, 0, st>>>(G->peers, G->world, G->rank, step, total, static_cast<const ScanCtrl*>(W.ctrl.p));
         k_group_wait_base<<<1, 1, 0, st>>>(G->ctl, G->rank, step);
         j->d->launches += 3;
         j->out_cap = G->match_cap;

@@ -109,6 +109,7 @@ struct ScanCtrl {
     unsigned int blk_cursor;       // bump allocator
     unsigned int overflow;         // pool exhausted
     unsigned int bad_offsets;      // the haystack offsets are not ascending, exceed text_bytes, or a haystack is >= 4 GiB
+    unsigned int carries;          // matches path: times a per-item u32 match count wrapped past 2^32 (count_carry)
 };
 
 struct ScanParams {
@@ -287,6 +288,20 @@ struct TextWin {
 };
 
 // ---- match emission --------------------------------------------------------------------
+// The matches path counts matches per item in 32 bits (counts, block headers and the item-relative indices k_gather /
+// k_expand place by).  A find_overlapping item that is not cut into segments can pass 2^32 matches; where its count
+// wraps, count_carry() records the carry -- finish_scan (dev_scan.cu) then reports the exact total, item_offs[n] +
+// carries * 2^32, and refuses the scan -- and raises `overflow`, so that no placement kernel writes by the wrapped
+// offsets.  The check sits where a count grows (emit, the event drain), never in a machine's step().
+DACH_HD void count_carry(const ScanParams& P) {
+#if defined(__CUDA_ARCH__)
+    asm volatile("red.global.add.u32 [%0], 1;" ::"l"(&P.ctrl->carries) : "memory");
+#else
+    ++P.ctrl->carries;
+#endif
+    P.ctrl->overflow = 1u;
+}
+
 struct Emitter {
     static constexpr int KIND = RK_MATCHES;
     uint32_t* blk;   // current block (nullptr when the pool is exhausted or nothing emitted yet)
@@ -315,7 +330,7 @@ struct Emitter {
             st_stream_u4(blk + BLK_SLOT_WORDS * (1 + fill), start, end, value, 0u);
         }
         fill = (fill + 1 == BLK_MATCHES) ? 0 : fill + 1;
-        ++count;
+        if (++count == 0) count_carry(P);
     }
     DACH_HD void finish(const ScanParams& P) { P.counts[item] = count; }
     DACH_HD bool stopped() const { return false; }
@@ -2294,7 +2309,9 @@ struct EventOps {
                     if (E.blk) st_stream_u2(E.blk + BLK_HDR_WORDS + 2 * E.fill, e.end, e.opos);
                     ++E.fill;
                     ++E.nev;
-                    E.count += MODE == M_OVERLAPPING ? qentry_len(P, Ev.opos, e.opos) : 1u;
+                    const uint32_t c = E.count + (MODE == M_OVERLAPPING ? qentry_len(P, Ev.opos, e.opos) : 1u);
+                    if (c < E.count) count_carry(P);
+                    E.count = c;
                 }
             }
         }

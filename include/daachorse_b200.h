@@ -141,13 +141,17 @@ size_t dach_dev_image_bytes(const dach_dev *dev); /* bytes resident in HBM for t
  *   text_bytes  total byte length of d_text (== offs[n]); the kernel never reads past it
  *   d_out       device pointer, capacity out_cap matches
  *   d_out_offs  device pointer, n+1 u64
- *   needed      host pointer; receives the total number of matches
+ *   needed      host pointer; receives the total number of matches (exact, also past 2^32)
  *   stream      cudaStream_t (NULL = default stream); the call synchronises the stream
  *               before returning
  *
  * Returns DACH_OUTPUT_OVERFLOW (and *needed) when out_cap is too small; nothing useful is
- * in d_out then.  DACH_MATCH_KIND_MISMATCH mirrors the crate's panics.  Charwise haystacks
- * must be valid UTF-8 (as &str guarantees in the crate). */
+ * in d_out then, and nothing at or past d_out + out_cap is written.  A haystack that yields
+ * 2^32 or more matches cannot be placed (per-haystack match indices are u32): the call
+ * returns DACH_INVALID_ARGUMENT with the exact *needed and writes no match; count such
+ * batches with dach_dev_count_batch / dach_dev_hist_batch.  Stream chunks, the host form and
+ * jobs behave the same.  DACH_MATCH_KIND_MISMATCH mirrors the crate's panics.  Charwise
+ * haystacks must be valid UTF-8 (as &str guarantees in the crate). */
 int dach_dev_scan_batch(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs,
                         uint64_t n, uint64_t text_bytes, dach_match *d_out, uint64_t out_cap,
                         uint64_t *d_out_offs, uint64_t *needed, void *stream);
@@ -253,7 +257,9 @@ int dach_hist_batch_host(dach_dev *dev, int mode, int key, const uint8_t *text, 
  *                   NULL for 0; d_out / d_out_offs may be peer-mapped memory of another GPU.
  *   dach_job_wait   blocks until the placement is done; status and *needed as dach_dev_scan_batch.
  * A job holds one scan at a time: scan -> place -> (wait) -> scan ...; the next dach_job_scan is
- * ordered after the previous placement by the library.  Options are read from the dach_dev. */
+ * ordered after the previous placement by the library.  Options are read from the dach_dev.
+ * A job keeps its dach_dev alive: dach_dev_free may come first (as a garbage collector may order
+ * it); the device image is then released by the last dach_job_free of that device. */
 typedef struct dach_job dach_job;
 int dach_job_create(dach_dev *dev, dach_job **out);
 void dach_job_free(dach_job *job);

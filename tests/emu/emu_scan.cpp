@@ -370,9 +370,10 @@ extern "C" int emu_scan_batch_wire(const uint8_t* wire, size_t wire_len, int cha
     // offsets (k_offsets_*), per-haystack offsets (k_hay_offsets) and gather (k_gather)
     std::vector<uint64_t> item_offs(n_items + 1, 0);
     for (uint64_t i = 0; i < n_items; ++i) item_offs[i + 1] = item_offs[i] + counts[i];
-    const uint64_t run = item_offs[n_items];
+    const uint64_t run = item_offs[n_items] + ((uint64_t)ctrl.carries << 32);  // finish_scan: exact past 2^32
     for (uint64_t h = 0; h <= n; ++h) out_offs[h] = seg ? item_offs[seg_first[h]] : item_offs[h];
     if (needed) *needed = run;
+    if (ctrl.carries) return DACH_INVALID_ARGUMENT;  // a haystack with 2^32 or more matches cannot be placed
     if (ctrl.overflow || run > out_cap) return DACH_OUTPUT_OVERFLOW;
     const uint32_t used_blocks = ctrl.blk_cursor < pool_blocks ? ctrl.blk_cursor : pool_blocks;
     uint32_t* out_words = reinterpret_cast<uint32_t*>(out);

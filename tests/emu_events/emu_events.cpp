@@ -183,9 +183,10 @@ extern "C" int emu_events_scan_wire(const uint8_t* wire, size_t wire_len, int mo
     // offsets (k_offsets_*), per-haystack offsets (k_final_offsets)
     std::vector<uint64_t> item_offs(n_items + 1, 0);
     for (uint64_t i = 0; i < n_items; ++i) item_offs[i + 1] = item_offs[i] + counts[i];
-    const uint64_t total = item_offs[n_items];
+    const uint64_t total = item_offs[n_items] + ((uint64_t)ctrl.carries << 32);  // finish_scan: exact past 2^32
     for (uint64_t h = 0; h <= n; ++h) out_offs[h] = seg ? item_offs[seg_first[h]] : item_offs[h];
     if (needed) *needed = total;
+    if (ctrl.carries) return DACH_INVALID_ARGUMENT;  // a haystack with 2^32 or more matches cannot be placed
     if (ctrl.overflow || total > out_cap) return DACH_OUTPUT_OVERFLOW;
     // k_expand: every event of every block, its list from output_pos of its slot along the parent links
     const uint32_t n_blocks = ctrl.blk_cursor < pool_blocks ? ctrl.blk_cursor : pool_blocks;

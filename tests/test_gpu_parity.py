@@ -581,6 +581,12 @@ def _group_case(world, devices):
     blobs = [g.handle for g in groups]
     for g in groups:
         g.connect(blobs)
+    sent32, sent64 = 0x5A5A5A5A, 0x5A5A5A5A5A5A5A5A
+    with torch.cuda.device(devices[0]):
+        m_all, o_all = groups[0].result(cap)  # rank 0's whole result buffers: nothing past `total` may be written
+        m_all.fill_(sent32)
+        o_all.fill_(sent64)
+        torch.cuda.synchronize()
     jobs, inputs, streams = [], [], []
     for r in range(world):
         dev = torch.device("cuda", devices[r])
@@ -609,8 +615,9 @@ def _group_case(world, devices):
             m, o = groups[0].result(total)
             assert total == whole.matches.shape[0]
             assert torch.equal(m, whole.matches) and torch.equal(o, whole.offsets)
-            m.zero_()
-            o.zero_()
+            assert bool((m_all[total:] == sent32).all())
+            m_all.fill_(sent32)
+            o_all.fill_(sent64)
             torch.cuda.synchronize()
     for g in groups:
         g.close()
