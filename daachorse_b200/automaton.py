@@ -480,6 +480,56 @@ class _Automaton:
                                                C.byref(total), st))
         return out
 
+    def doc_counts_host(self, mode, text, offs, key="value", out=None, device=None):
+        """In how many haystacks of the batch each pattern occurs (document frequency), host buffers in and out:
+        ``np.uint64`` counts, added into ``out`` if given (zeros otherwise).  Bin k counts the haystacks with at least
+        one match of key k -- keys as in ``pattern_counts_host``.  No match list; on an error ``out`` is unchanged."""
+        text, offs, n = self._host_batch_args(mode, text, offs)
+        need = self._hist_len(key)
+        if out is None:
+            out = np.zeros(need, dtype=np.uint64)
+        elif out.dtype != np.uint64 or out.ndim != 1 or not out.flags.c_contiguous or not out.flags.writeable:
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "out must be a writable contiguous 1-d uint64 array")
+        L = _lib.load()
+        d = self.device_handle(device)
+        total = C.c_uint64()
+        _check(L.dach_df_batch_host(d, mode, HIST_KEYS[key], _ptr(text), C.c_void_p(offs.ctypes.data), n, _ptr(out), out.size,
+                                    C.byref(total)))
+        return out
+
+    def doc_counts_device(self, mode, text, offs, key="value", out=None, stream=None):
+        """Device-resident form of ``doc_counts_host``: ``text`` / ``offs`` as in ``scan_batch_device``; returns the
+        int64 CUDA counts, added into ``out`` if given (zeros otherwise) -- calls on consecutive batches accumulate a
+        corpus on the device."""
+        import torch
+
+        self._assert_mode(mode)
+        dev = text.device.index if text.device.index is not None else torch.cuda.current_device()
+        need = self._hist_len(key)
+        if out is None:
+            out = torch.zeros(need, dtype=torch.int64, device=text.device)
+        _check_device_batch(text, offs, dev, hist=out, hist_len=need)
+        d = self.device_handle(dev)
+        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
+        total = C.c_uint64()
+        _check(_lib.load().dach_dev_df_batch(d, mode, HIST_KEYS[key], C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()),
+                                             offs.numel() - 1, text.numel(), C.c_void_p(out.data_ptr()), out.numel(),
+                                             C.byref(total), st))
+        return out
+
+    def last_doc_windows(self, device=None):
+        """``(windows, rescans)`` of the last ``doc_counts_*`` call on this device: the windows the batch was scanned
+        in, and how many of them overflowed the pair sets (option ``df_pairs``) and were scanned again as halves."""
+        w, r = C.c_uint64(), C.c_uint64()
+        _check(_lib.load().dach_dev_last_df_windows(self.device_handle(device), C.byref(w), C.byref(r)))
+        return w.value, r.value
+
+    def value_doc_counts_batch(self, haystacks, mode=None):
+        """Haystacks containing each value: ``np.uint64[max value + 1]`` (for ``new`` automata: per pattern);
+        ``mode=None`` as in ``count_batch``."""
+        blob, offs = _pack(list(haystacks), self._charwise)
+        return self.doc_counts_host(self._default_mode(mode), blob, offs, key="value")
+
     def value_counts_batch(self, haystacks, mode=None):
         """Occurrences per value over all haystacks: ``np.uint64[max value + 1]`` (for ``new`` automata: per pattern);
         ``mode=None`` as in ``count_batch``."""

@@ -13,9 +13,10 @@
 //       k_scan_duo<MODE>        StdMachine3 with two haystacks per lane (option kernel = 4; measured slower)
 //       k_scan<CHARWISE, MODE>  lane per haystack, reference-shaped loop: automata above 2^24 slots, find_iter with
 //                               an empty pattern, and option kernel = 0
-//     k_scan_machine_rk / k_scan_rk  the same machines / loops with a COUNT, FIRST or HIST sink (dach_dev_count_batch,
-//                               dach_dev_first_batch, dach_dev_hist_batch), followed by k_count_hay / k_first_hay
-//                               (per-haystack results) or k_hist_heads / k_hist_fold (per-pattern counts)
+//     k_scan_machine_rk / k_scan_rk  the same machines / loops with a COUNT, FIRST, HIST or DF sink (dach_dev_count_batch,
+//                               dach_dev_first_batch, dach_dev_hist_batch, dach_dev_df_batch), followed by k_count_hay /
+//                               k_first_hay (per-haystack results), k_hist_heads / k_hist_fold (per-pattern counts) or
+//                               k_df_expand / k_df_add / k_df_clear (document frequencies, window by window)
 //     k_offsets_*               exclusive scan of the per-item match counts
 //     k_blk_index               pool blocks listed in output order (large batches)
 //   phase 2
@@ -58,12 +59,18 @@ namespace dach {
 constexpr int kMaxThreads = 1024;
 constexpr int kMaxDevices = 64;
 constexpr uint32_t kRootBytes = 1024;  // 256 x u32 at the front of dynamic shared memory
+// DF: pairs per window by default (option df_pairs).  DESIGN.md section 4.9 measures the distinct pairs per MiB of
+// text (tools/lane_stats.py --pairs): at most 84 k (C2), so the largest slice cut_slices makes on the bench workloads
+// (540 MiB of C3 find_iter, 26 k pairs per MiB) fits in one window.  Cost: 2 sets x 2^25 entries x 12 B = 768 MiB.
+constexpr int64_t kDefaultDfPairs = 1 << 24;
 
 // the result sink of each result kind
 template <int RK>
 using SinkOf = typename std::conditional<
     RK == RK_COUNT, CountSink,
-    typename std::conditional<RK == RK_FIRST, FirstSink, typename std::conditional<RK == RK_HIST, HistSink, Emitter>::type>::type>::type;
+    typename std::conditional<
+        RK == RK_FIRST, FirstSink,
+        typename std::conditional<RK == RK_HIST, HistSink, typename std::conditional<RK == RK_DF, DfSink, Emitter>::type>::type>::type>::type;
 
 template <bool CHARWISE, int MODE, class SINK>
 __device__ __forceinline__ void scan_items(const ScanParams& P) {
@@ -96,7 +103,7 @@ template <bool CHARWISE, int MODE>
 __global__ void __launch_bounds__(kMaxThreads, 1) k_scan(ScanParams P) {
     scan_items<CHARWISE, MODE, Emitter>(P);
 }
-// COUNT / FIRST (result kind RK) on the lane-per-haystack loops
+// COUNT / FIRST / HIST / DF (result kind RK) on the lane-per-haystack loops
 template <bool CHARWISE, int MODE, int RK>
 __global__ void __launch_bounds__(kMaxThreads, 1) k_scan_rk(ScanParams P) {
     scan_items<CHARWISE, MODE, SinkOf<RK>>(P);
@@ -862,6 +869,49 @@ __global__ void __launch_bounds__(256) k_hist_fold(const unsigned long long* rec
     add_block_total(added, total);
 }
 
+// ---- DF: the window's (haystack, key) pairs, then one per pair into the document frequencies ------------------------
+// k_df_expand  (lane machines) every (haystack, slot) pair of the scan: the records its events reported -- the head
+//              opos[slot], with CHAIN (find_overlapping) its whole parent chain, exactly what k_hist_fold<true> adds
+//              to -- each mapped to its key and put into the key set as (haystack, key).
+// k_df_add     df_acc[key] += 1 and *total += 1 per (haystack, key) pair of the window.
+// Both do nothing once the window has overflowed (either set took more than df_pairs pairs), so df_acc only ever
+// holds whole windows; k_df_clear then empties both sets for the next window by their lists.
+template <bool CHAIN>
+__global__ void __launch_bounds__(256) k_df_expand(ScanParams P) {
+    const volatile unsigned int* over = &P.ctrl->overflow;
+    if (*over) return;
+    const unsigned int n = *P.df_slots.n;
+    for (unsigned int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const unsigned long long pair = P.df_slots.keys[P.df_slots.list[i]];
+        const unsigned long long hay = pair & 0xffffffff00000000ull;
+        uint32_t j = P.opos_tab[(uint32_t)pair];
+        while (j) {
+            const uint4 o = P.outputs[j - 1];
+            if (df_insert(P.df_keys, hay | (P.df_key_value ? o.x : j - 1), P.ctrl) == DF_FULL) return;
+            j = CHAIN ? o.z : 0u;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) k_df_add(DfSet keys, const ScanCtrl* ctrl, unsigned long long* df_acc, unsigned long long* total) {
+    if (ctrl->overflow) return;
+    const unsigned int n = *keys.n;
+    if (blockIdx.x == 0 && threadIdx.x == 0) *total += n;
+    for (unsigned int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        red_add_u64(df_acc + (uint32_t)keys.keys[keys.list[i]], 1);
+}
+
+__global__ void __launch_bounds__(256) k_df_clear(DfSet a, DfSet b) {
+    const unsigned int na = *a.n, nb = *b.n;  // both at most mask + 1 (one list position per taken entry)
+    for (unsigned int i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) a.keys[a.list[i]] = DF_EMPTY;
+    for (unsigned int i = blockIdx.x * blockDim.x + threadIdx.x; i < nb; i += gridDim.x * blockDim.x) b.keys[b.list[i]] = DF_EMPTY;
+}
+
+// df[i] += acc[i]: a call's counts reach the caller's buffer only once all its windows are done
+__global__ void __launch_bounds__(256) k_df_commit(const unsigned long long* acc, unsigned long long* df, uint64_t n) {
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) df[i] += acc[i];
+}
+
 }  // namespace dach
 
 // ------------------------------------------------------------------------------------------
@@ -1016,7 +1066,11 @@ struct dach_dev {
     // HIST on the lane machines: events of the leading compact slots are counted in shared memory per CTA (4 B
     // each, next to the hot records and the queues) before they reach global memory.  0 = off.
     int64_t opt_hist_smem = 1024;
-    int64_t opt_slice_ramp = 1;      // host path: small slices at the head and the tail of a batch
+    // DF: the most (haystack, state) and (haystack, key) pairs one window may hold; both sets take the next power of
+    // two at or above twice that many entries, 12 B each.  At least max(compact slots, output records), so that one
+    // haystack always fits.  The default: kDefaultDfPairs.
+    int64_t opt_df_pairs = kDefaultDfPairs;
+    int64_t opt_slice_ramp = 1;     // host path: small slices at the head and the tail of a batch
     int64_t opt_tail_seg = 0;        // cut only the last 2 x lanes haystacks of a large batch (off by default)
     int64_t opt_gather_ordered = 1;  // copy pool blocks in output order (sequential writes)
     int64_t opt_gather_u = 4;     // pooled blocks in flight per warp of k_gather (2, 4 or 8)
@@ -1036,6 +1090,12 @@ struct dach_dev {
     cudaEvent_t ev_ref = nullptr;  // time zero of dach_job_times (recorded at the first job scan)
     double last_scan_ms = 0, last_total_ms = 0;
     uint64_t last_h2d = 0, last_d2h = 0;
+    // DF (dach_dev_df_batch / dach_df_batch_host, both under mu): the two pair sets, shared by every window of both
+    // forms -- each window is finished before the next is enqueued -- and the call's document frequencies
+    DevBuf df_tab[2], df_list[2], df_n, df_acc;
+    uint32_t df_mask = 0, df_limit = 0;
+    bool df_clean = false;  // both sets are empty (false after a failed window: the next call empties them in full)
+    uint64_t last_df_windows = 0, last_df_rescans = 0;
     // the handle's owner plus one per live job: dach_dev_free may come before the jobs are freed (a garbage collector
     // finalises in any order), and the jobs still read the image and d->device until then
     std::atomic<int> refs{1};
@@ -1204,19 +1264,19 @@ cudaError_t launch_scan_rk_t(const ScanParams& P, int grid, int threads, size_t 
 }
 
 // which: 3 StdMachine3 (bytewise Standard), 1 LmMachine / CwMachine (by the automaton), 0 lane per haystack.
-// FIRST only runs M_OVERLAPPING (Standard) and M_LEFTMOST: the caller folds the Standard modes.  HIST runs all of
-// COUNT's kernels.
+// FIRST only runs M_OVERLAPPING (Standard) and M_LEFTMOST: the caller folds the Standard modes.  HIST and DF run all
+// of COUNT's kernels.
 template <int RK>
 cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
     if (which == 3) {
         switch (mode) {
             case M_FIND:
-                if constexpr (RK == RK_COUNT || RK == RK_HIST)
+                if constexpr (RK != RK_FIRST)
                     return P.hot_entries ? launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, RK, true>(P, grid, threads, smem, st)
                                          : launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, RK, false>(P, grid, threads, smem, st);
                 break;
             case M_NO_SUFFIX:
-                if constexpr (RK == RK_COUNT || RK == RK_HIST)
+                if constexpr (RK != RK_FIRST)
                     return P.hot_entries ? launch_rk_t<StdMachine3<M_NO_SUFFIX>, Lane3, M_NO_SUFFIX, RK, true>(P, grid, threads, smem, st)
                                          : launch_rk_t<StdMachine3<M_NO_SUFFIX>, Lane3, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
                 break;
@@ -1229,10 +1289,10 @@ cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int gri
     if (which == 1 && cw) {
         switch (mode) {
             case M_FIND:
-                if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_rk_t<CwMachine<M_FIND>, LaneCw, M_FIND, RK, false>(P, grid, threads, smem, st);
+                if constexpr (RK != RK_FIRST) return launch_rk_t<CwMachine<M_FIND>, LaneCw, M_FIND, RK, false>(P, grid, threads, smem, st);
                 break;
             case M_NO_SUFFIX:
-                if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_rk_t<CwMachine<M_NO_SUFFIX>, LaneCw, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
+                if constexpr (RK != RK_FIRST) return launch_rk_t<CwMachine<M_NO_SUFFIX>, LaneCw, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
                 break;
             case M_OVERLAPPING: return launch_rk_t<CwMachine<M_OVERLAPPING>, LaneCw, M_OVERLAPPING, RK, false>(P, grid, threads, smem, st);
             case M_LEFTMOST: return launch_rk_t<CwMachine<M_LEFTMOST>, LaneCw, M_LEFTMOST, RK, false>(P, grid, threads, smem, st);
@@ -1241,13 +1301,13 @@ cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int gri
     }
     if (which == 1) return mode == M_LEFTMOST ? launch_rk_t<LmMachine, LaneLm, M_LEFTMOST, RK, false>(P, grid, threads, smem, st) : cudaErrorInvalidValue;
     switch ((cw ? 4 : 0) + mode) {
-        case 0: if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_scan_rk_t<false, M_FIND, RK>(P, grid, threads, smem, st); break;
+        case 0: if constexpr (RK != RK_FIRST) return launch_scan_rk_t<false, M_FIND, RK>(P, grid, threads, smem, st); break;
         case 1: return launch_scan_rk_t<false, M_OVERLAPPING, RK>(P, grid, threads, smem, st);
-        case 2: if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_scan_rk_t<false, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
+        case 2: if constexpr (RK != RK_FIRST) return launch_scan_rk_t<false, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
         case 3: return launch_scan_rk_t<false, M_LEFTMOST, RK>(P, grid, threads, smem, st);
-        case 4: if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_scan_rk_t<true, M_FIND, RK>(P, grid, threads, smem, st); break;
+        case 4: if constexpr (RK != RK_FIRST) return launch_scan_rk_t<true, M_FIND, RK>(P, grid, threads, smem, st); break;
         case 5: return launch_scan_rk_t<true, M_OVERLAPPING, RK>(P, grid, threads, smem, st);
-        case 6: if constexpr (RK == RK_COUNT || RK == RK_HIST) return launch_scan_rk_t<true, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
+        case 6: if constexpr (RK != RK_FIRST) return launch_scan_rk_t<true, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
         case 7: return launch_scan_rk_t<true, M_LEFTMOST, RK>(P, grid, threads, smem, st);
     }
     return cudaErrorInvalidValue;
@@ -1860,9 +1920,21 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
     return DACH_OK;
 }
 
-// ---- COUNT / FIRST / HIST: the scan of a batch and its results on one stream.  No synchronisation. ----------------
+// DF: set i (0: (haystack, slot) pairs, 1: (haystack, key) pairs) as the kernels see it
+DfSet df_set(dach_dev* d, int i) {
+    DfSet S;
+    S.keys = static_cast<unsigned long long*>(d->df_tab[i].p);
+    S.list = static_cast<uint32_t*>(d->df_list[i].p);
+    S.n = static_cast<unsigned int*>(d->df_n.p) + i;
+    S.mask = d->df_mask;
+    S.limit = d->df_limit;
+    return S;
+}
+
+// ---- COUNT / FIRST / HIST / DF: the scan of a batch and its results on one stream.  No synchronisation. -----------
 // rk = RK_COUNT: d_counts (n x u64); RK_FIRST: d_first (n tuples), d_found (n x u8); RK_HIST: added into d_hist by
-// `key` (DACH_KEY_OUTPUT / DACH_KEY_VALUE; the caller has checked its size).  The total (matches, or haystacks with a
+// `key` (DACH_KEY_OUTPUT / DACH_KEY_VALUE; the caller has checked its size); RK_DF: one window (df_windows), added
+// into d_hist by `key` unless W.pinned->ctrl.overflow is set once W.ev_placed has completed.  The total (matches, or haystacks with a
 // match) lands in W.pinned->total_rk once W.ev_placed has completed.  No block pool, no offsets, no gather: options
 // kernel = 1, 2, 4 run StdMachine3 here (kernel = 0: the lane-per-haystack kernels).
 int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
@@ -1911,7 +1983,7 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             }
         }
         const uint64_t n_tiles = (n + kScanTile - 1) / kScanTile;
-        if (rk != RK_HIST && !ensure(W.items_rk, n_items_max * (rk == RK_FIRST ? 16 : 8))) return DACH_CUDA_ERROR;
+        if ((rk == RK_COUNT || rk == RK_FIRST) && !ensure(W.items_rk, n_items_max * (rk == RK_FIRST ? 16 : 8))) return DACH_CUDA_ERROR;
         if (seg && (!ensure(W.tiles, n_tiles * 8) || !ensure(W.nseg, n * 4) || !ensure(W.seg_first, (n + 1) * 8) ||
                     !ensure(W.item_hay, n_items_max * 4) || !ensure(W.item_beg, n_items_max * 4) || !ensure(W.n_items_dev, 8)))
             return DACH_CUDA_ERROR;
@@ -1931,6 +2003,11 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             P.rec_hist = static_cast<unsigned long long*>(W.rec_hist.p);
             P.hist_smem = hist_k;
         }
+        if (rk == RK_DF) {  // the sets are empty here (df_prepare, then k_df_clear after every window)
+            P.df_key_value = key == DACH_KEY_VALUE;
+            P.df_slots = df_set(d, 0);
+            P.df_keys = df_set(d, 1);
+        }
         const size_t smem = plan_smem(d, P, machine, std3, threads, ctas_per_sm, 1, hist_k);
         k_check_offsets<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_offs, n, (uint64_t)(text_end - d_text), P.ctrl);
         ++d->launches;
@@ -1940,6 +2017,7 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         const int t = machine ? std::min(threads, 1024) : threads;
         if (!cuda_ok(rk == RK_COUNT  ? launch_rk<RK_COUNT>(which, d->charwise, mmode, P, grid, t, smem, st)
                      : rk == RK_HIST ? launch_rk<RK_HIST>(which, d->charwise, mmode, P, grid, t, smem, st)
+                     : rk == RK_DF   ? launch_rk<RK_DF>(which, d->charwise, mmode, P, grid, t, smem, st)
                                      : launch_rk<RK_FIRST>(which, d->charwise, mmode, P, grid, t, smem, st),
                      "k_scan launch"))
             return DACH_CUDA_ERROR;
@@ -1959,12 +2037,24 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             else
                 k_hist_fold<false><<<fb, 256, 0, st>>>(P.rec_hist, d->d_outputs, d->n_outputs, key, hist, total);
             ++d->launches;
+        } else if (rk == RK_DF) {
+            // lane machines: (haystack, slot) -> (haystack, key); then the window's pairs into d_hist (the call's
+            // accumulator) unless it overflowed, and both sets emptied for the next window
+            const unsigned fb = (unsigned)(8 * d->sm_count);
+            if (machine && mmode == M_OVERLAPPING)
+                k_df_expand<true><<<fb, 256, 0, st>>>(P);
+            else if (machine)
+                k_df_expand<false><<<fb, 256, 0, st>>>(P);
+            k_df_add<<<fb, 256, 0, st>>>(P.df_keys, P.ctrl, reinterpret_cast<unsigned long long*>(d_hist), total);
+            k_df_clear<<<fb, 256, 0, st>>>(P.df_slots, P.df_keys);
+            d->launches += machine ? 3 : 2;
+            if (!cuda_ok(cudaMemsetAsync(d->df_n.p, 0, 8, st), "memset pair counts")) return DACH_CUDA_ERROR;
         } else if (rk == RK_COUNT)
             k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(d_counts), total);
         else
             k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(d_first), d_found, total);
-        if (rk != RK_HIST) d->launches += 2;  // the scan and k_count_hay / k_first_hay
-        else ++d->launches;                   // the scan
+        if (rk == RK_COUNT || rk == RK_FIRST) d->launches += 2;  // the scan and k_count_hay / k_first_hay
+        else ++d->launches;                                    // the scan
         if (!cuda_ok(cudaGetLastError(), "kernel launch")) return DACH_CUDA_ERROR;
     } else {
         cudaEventRecord(W.ev[1], st);
@@ -2135,6 +2225,167 @@ int hist_batch_host_impl(dach_dev* d, int mode, int key, const uint8_t* text, co
     return DACH_OK;
 }
 
+// ---- DF ---------------------------------------------------------------------------------------------------------
+// Both pair sets sized by option df_pairs and empty, and the call's accumulator (n_df x u64) zeroed, on stream st
+int df_prepare(dach_dev* d, uint64_t n_df, cudaStream_t st) {
+    const uint64_t limit = std::min<uint64_t>(std::max<uint64_t>({(uint64_t)std::max<int64_t>(d->opt_df_pairs, 1), d->n_cslots, d->n_outputs}), 1ull << 30);
+    uint64_t cap = 2;
+    while (cap < 2 * limit) cap <<= 1;
+    if (cap - 1 != d->df_mask || !d->df_tab[0].p) d->df_clean = false;
+    d->df_mask = (uint32_t)(cap - 1);
+    d->df_limit = (uint32_t)limit;
+    if (!ensure(d->df_acc, n_df * 8) || !cuda_ok(cudaMemsetAsync(d->df_acc.p, 0, n_df * 8, st), "memset document frequencies"))
+        return DACH_CUDA_ERROR;
+    if (!d->df_clean) {
+        for (int i = 0; i < 2; ++i)
+            if (!ensure(d->df_tab[i], cap * 8) || !ensure(d->df_list[i], cap * 4) ||
+                !cuda_ok(cudaMemsetAsync(d->df_tab[i].p, 0xff, cap * 8, st), "memset pair set"))
+                return DACH_CUDA_ERROR;
+        if (!ensure(d->df_n, 8) || !cuda_ok(cudaMemsetAsync(d->df_n.p, 0, 8, st), "memset pair counts")) return DACH_CUDA_ERROR;
+        d->df_clean = true;
+    }
+    return cuda_ok(cudaStreamSynchronize(st), "prepare pair sets") ? DACH_OK : DACH_CUDA_ERROR;
+}
+
+// DF of haystacks [first, last) of a batch whose host offsets are `offs` and whose device offsets from haystack
+// `first` on are d_offs, on W / st: windows of at most *win haystacks, each scanned, expanded and -- unless it
+// overflowed -- added into d->df_acc before the next is enqueued.  A window that overflows is scanned again as two
+// halves, and *win keeps the smaller size for the rest of the call.  A window of one haystack cannot overflow: it
+// holds at most n_cslots distinct states and n_outputs distinct keys, and df_limit is at least both.
+int df_windows(dach_dev* d, Workspace& W, int mode, int key, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
+               const uint64_t* d_offs, const uint64_t* offs, uint64_t first, uint64_t last, cudaStream_t st, uint64_t* win, uint64_t* sum) {
+    for (uint64_t a = first; a < last;) {
+        const uint64_t b = last - a <= *win ? last : a + *win;
+        d->df_clean = false;
+        int rc = enqueue_rk(d, W, RK_DF, mode, d_text, text_lo, text_end, offs[b] - offs[a], d_offs + (a - first), b - a, nullptr, nullptr,
+                            nullptr, st, key, static_cast<uint64_t*>(d->df_acc.p));
+        if (rc) return rc;
+        d->df_clean = true;  // k_df_clear and the counters' reset are enqueued
+        uint64_t t = 0;
+        rc = finish_rk(d, W, &t);
+        if (rc) return rc;
+        if (W.pinned->ctrl.overflow) {
+            if (b - a == 1) {
+                set_error("document frequencies: one haystack overflowed the pair sets");
+                return DACH_CUDA_ERROR;
+            }
+            *win = (b - a + 1) / 2;
+            ++d->last_df_rescans;
+            continue;
+        }
+        ++d->last_df_windows;
+        *sum += t;
+        a = b;
+    }
+    return DACH_OK;
+}
+
+// DF of a device batch: the offsets come to the host once (8 B per haystack) to be checked and cut into the slices of
+// dach_scan_batch_host; the windows add into d->df_acc, which reaches d_df only when all of them are done
+int df_batch_dev_impl(dach_dev* d, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                      uint64_t* d_df, uint64_t n_df, uint64_t* total, cudaStream_t st) {
+    std::lock_guard<std::mutex> lk(d->mu);
+    DeviceGuard g(d->device);
+    if (!g.ok) return DACH_CUDA_ERROR;
+    d->last_h2d = d->last_d2h = 0;
+    d->last_df_windows = d->last_df_rescans = 0;
+    if (total) *total = 0;
+    if (n == 0) return DACH_OK;
+    if (n > 0xfffffff0ull) {
+        set_error("too many haystacks in one batch (max 2^32-16)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    std::vector<uint64_t> offs(n + 1);
+    if (!cuda_ok(cudaMemcpyAsync(offs.data(), d_offs, (n + 1) * 8, cudaMemcpyDeviceToHost, st), "D2H offsets") ||
+        !cuda_ok(cudaStreamSynchronize(st), "D2H offsets"))
+        return DACH_CUDA_ERROR;
+    d->last_d2h = (n + 1) * 8;
+    int rc = check_host_offsets(offs.data(), n);
+    if (rc) return rc;
+    if (offs[n] > text_bytes) {
+        set_error("haystack offsets must be inside text_bytes");
+        return DACH_INVALID_ARGUMENT;
+    }
+    rc = df_prepare(d, n_df, st);
+    if (rc) return rc;
+    const std::vector<Slice> slices = cut_slices(d, mode, offs.data(), n);
+    uint64_t win = ~0ull, sum = 0;
+    for (const Slice& s : slices) {
+        rc = df_windows(d, d->ws, mode, key, d_text, d_text, d_text + text_bytes, d_offs + s.first, offs.data(), s.first, s.last, st, &win, &sum);
+        if (rc) return rc;
+    }
+    if (n_df) {
+        k_df_commit<<<(unsigned)std::min<uint64_t>((n_df + 255) / 256, 8 * d->sm_count), 256, 0, st>>>(
+            static_cast<const unsigned long long*>(d->df_acc.p), reinterpret_cast<unsigned long long*>(d_df), n_df);
+        ++d->launches;
+        if (!cuda_ok(cudaGetLastError(), "kernel launch") || !cuda_ok(cudaStreamSynchronize(st), "add document frequencies"))
+            return DACH_CUDA_ERROR;
+    }
+    if (total) *total = sum;
+    return DACH_OK;
+}
+
+// DF of a host-buffer batch: the slices of dach_scan_batch_host, each cut into windows; d->df_acc comes back once and
+// is added into the caller's
+int df_batch_host_impl(dach_dev* d, int mode, int key, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* df, uint64_t n_df,
+                       uint64_t* total) {
+    if (!d || !offs || (n_df && !df)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    int rc = check_hist(d, key, n_df);
+    if (rc) return rc;
+    rc = check_mode(d, mode);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(d->mu);
+    DeviceGuard g(d->device);
+    if (!g.ok) return DACH_CUDA_ERROR;
+    d->last_h2d = d->last_d2h = 0;
+    d->last_df_windows = d->last_df_rescans = 0;
+    if (total) *total = 0;
+    if (n == 0) return DACH_OK;
+    rc = check_host_offsets(offs, n);
+    if (rc) return rc;
+    struct Drain {  // no exit may leave copies of the caller's buffers in flight
+        dach_dev* d;
+        ~Drain() {
+            for (Workspace& w : d->slot)
+                if (w.stream) cudaStreamSynchronize(w.stream);
+        }
+    } drain_on_exit{d};
+    const std::vector<Slice> slices = cut_slices(d, mode, offs, n);
+    for (Workspace& w : d->slot)
+        if (!w.init(true)) return DACH_CUDA_ERROR;
+    rc = df_prepare(d, n_df, d->slot[0].stream);
+    if (rc) return rc;
+    double t_reuse = 0;
+    auto issue_h2d = [&](size_t k) -> bool {
+        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
+    };
+    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
+    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
+    uint64_t win = ~0ull, sum = 0;
+    for (size_t k = 0; k < slices.size(); ++k) {
+        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
+        Workspace& W = d->slot[k % dach_dev::kSlots];
+        const Slice& s = slices[k];
+        const uint64_t tb = offs[s.last] - offs[s.first];
+        const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
+        rc = df_windows(d, W, mode, key, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb,
+                        static_cast<const uint64_t*>(W.offs.p), offs, s.first, s.last, W.stream, &win, &sum);
+        if (rc) return rc;
+    }
+    for (Workspace& w : d->slot)
+        if (!cuda_ok(cudaStreamSynchronize(w.stream), "scan")) return DACH_CUDA_ERROR;
+    std::vector<uint64_t> h(n_df);
+    if (n_df && !cuda_ok(cudaMemcpy(h.data(), d->df_acc.p, n_df * 8, cudaMemcpyDeviceToHost), "D2H document frequencies"))
+        return DACH_CUDA_ERROR;
+    d->last_d2h = n_df * 8;
+    for (uint64_t i = 0; i < n_df; ++i) df[i] += h[i];
+    if (total) *total = sum;
+    return DACH_OK;
+}
+
 // maps every exception to a status: nothing may unwind through the C ABI
 template <class F>
 int guarded(F&& f) {
@@ -2243,6 +2494,8 @@ void dach_dev_free(dach_dev* d) {
     if (d->ev_ref) cudaEventDestroy(d->ev_ref);
     d->ws.release();
     for (Workspace& w : d->slot) w.release();
+    for (DevBuf* b : {&d->df_tab[0], &d->df_tab[1], &d->df_list[0], &d->df_list[1], &d->df_n, &d->df_acc})
+        if (b->p) cudaFree(b->p);
     delete d;
 }
 
@@ -2361,6 +2614,33 @@ int dach_dev_hist_batch(dach_dev* d, int mode, int key, const uint8_t* d_text, c
 int dach_hist_batch_host(dach_dev* d, int mode, int key, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* hist,
                          uint64_t n_hist, uint64_t* total) {
     return guarded([&]() -> int { return hist_batch_host_impl(d, mode, key, text, offs, n, hist, n_hist, total); });
+}
+
+int dach_dev_df_batch(dach_dev* d, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                      uint64_t* d_df, uint64_t n_df, uint64_t* total, void* stream) {
+    if (!d || !d_offs || (n_df && !d_df)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    int rc = check_hist(d, key, n_df);
+    if (rc) return rc;
+    rc = check_mode(d, mode);
+    if (rc) return rc;
+    return guarded([&]() -> int {
+        return df_batch_dev_impl(d, mode, key, d_text, d_offs, n, text_bytes, d_df, n_df, total, static_cast<cudaStream_t>(stream));
+    });
+}
+
+int dach_df_batch_host(dach_dev* d, int mode, int key, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* df,
+                       uint64_t n_df, uint64_t* total) {
+    return guarded([&]() -> int { return df_batch_host_impl(d, mode, key, text, offs, n, df, n_df, total); });
+}
+
+int dach_dev_last_df_windows(const dach_dev* d, uint64_t* windows, uint64_t* rescans) {
+    if (!d) return DACH_INVALID_ARGUMENT;
+    if (windows) *windows = d->last_df_windows;
+    if (rescans) *rescans = d->last_df_rescans;
+    return DACH_OK;
 }
 
 // ---- asynchronous jobs ------------------------------------------------------------------------------
@@ -2757,6 +3037,8 @@ int dach_dev_set_option(dach_dev* d, const char* name, int64_t value) {
         d->opt_hot_entries = value;
     else if (k == "hist_smem")
         d->opt_hist_smem = value;
+    else if (k == "df_pairs")
+        d->opt_df_pairs = value;
     else if (k == "l2_hints") {
         d->opt_l2_hints = value;
         DeviceGuard g(d->device);

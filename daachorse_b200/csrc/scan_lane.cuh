@@ -16,8 +16,8 @@
 //   - StdMachine3  the default (kernel=3): no probe-state flags, one stop bit, cursor = address word, records from
 //                  the hot-first image (optionally its front from shared memory); probe / resolve are separate so
 //                  that k_scan_duo can keep two fetches in flight; serves stream chunks
-//   - SinkOps      COUNT / FIRST / HIST on StdMachine3, LmMachine, CwMachine: their drain() / begin_item() for
-//                  the other result kinds (sinks: Emitter, CountSink, FirstSink, HistSink)
+//   - SinkOps      COUNT / FIRST / HIST / DF on StdMachine3, LmMachine, CwMachine: their drain() / begin_item()
+//                  for the other result kinds (sinks: Emitter, CountSink, FirstSink, HistSink, DfSink)
 //   - EventOps     the matches path of StdMachine3: events stored into event blocks (EventSink), expanded after
 //                  the scan by k_expand
 //
@@ -112,6 +112,19 @@ struct ScanCtrl {
     unsigned int carries;          // matches path: times a per-item u32 match count wrapped past 2^32 (count_carry)
 };
 
+// DF: an open-addressing set of u64 pairs (haystack << 32 | slot or key) in device memory.  `keys` has mask + 1
+// entries (a power of two, at least twice `limit`), DF_EMPTY where free; `list` holds the positions of the
+// taken entries in the order they were taken (*n of them), so a window's pairs can be walked -- and the
+// set emptied again -- without touching the rest of the table.  More than `limit` pairs overflow the window.
+constexpr unsigned long long DF_EMPTY = ~0ull;
+struct DfSet {
+    unsigned long long* keys;
+    uint32_t* list;
+    unsigned int* n;
+    uint32_t mask;
+    uint32_t limit;
+};
+
 struct ScanParams {
     // automaton image
     const uint4* rec;
@@ -159,13 +172,17 @@ struct ScanParams {
     unsigned long long* slot_hist;
     unsigned long long* rec_hist;
     uint32_t hist_smem;
+    // DF (DfSink): the window's distinct (haystack, compact slot) pairs (lane machines) and (haystack, key)
+    // pairs (lane per haystack, and k_df_expand from the slot pairs); df_key_value: the key is the value
+    uint32_t df_key_value;
+    DfSet df_slots, df_keys;
 };
 
 // What a scan produces (compile time): every match (Emitter), the number of matches (CountSink), the first
-// match and whether there is one (FirstSink), or the matches per output record of the whole batch (HistSink).
-// The lane machines and the lane-per-haystack loops are the same for all four; the sink and, for FIRST, the
-// stop rule differ.
-constexpr int RK_MATCHES = 0, RK_COUNT = 1, RK_FIRST = 2, RK_HIST = 3;
+// match and whether there is one (FirstSink), the matches per output record of the whole batch (HistSink),
+// or the distinct (haystack, state / key) pairs of the batch (DfSink).  The lane machines and the
+// lane-per-haystack loops are the same for all five; the sink and, for FIRST, the stop rule differ.
+constexpr int RK_MATCHES = 0, RK_COUNT = 1, RK_FIRST = 2, RK_HIST = 3, RK_DF = 4;
 
 // L2 eviction policies (64-bit descriptors made once per device by k_make_policies, dev_scan.cu):
 //   [0] automaton image (records, output_pos, outputs, mapper): evict_last -- the scan is latency-bound on
@@ -498,6 +515,82 @@ DACH_HD void emit_chain(const ScanParams& P, HistSink&, uint32_t opos, uint32_t)
     }
 }
 
+// DF: put `pair` into set S (linear probing from a mixed hash).  DF_NEW: it was not there (its position is
+// appended to S.list); DF_OLD: it was; DF_FULL: the window overflowed -- S took more than S.limit pairs, or
+// every entry is taken -- and ctrl->overflow is raised.  A caller that sees DF_FULL stops inserting.  Once a
+// window has overflowed, the other lanes go on inserting until each meets the flag: a probe longer than 16
+// entries reads it (below the load limit the table is at most half full, and such probes are rare), so no
+// insert walks the whole of a table that lanes keep filling.
+constexpr int DF_OLD = 0, DF_NEW = 1, DF_FULL = 2;
+DACH_HD int df_insert(const DfSet& S, unsigned long long pair, ScanCtrl* ctrl) {
+    unsigned long long h = pair;
+    h ^= h >> 33;
+    h *= 0xff51afd7ed558ccdull;
+    h ^= h >> 33;
+    uint32_t at = (uint32_t)h & S.mask;
+    for (uint32_t probe = 0; probe <= S.mask; ++probe, at = (at + 1) & S.mask) {
+        if ((probe & 15u) == 15u && *static_cast<volatile unsigned int*>(&ctrl->overflow)) return DF_FULL;
+#if defined(__CUDA_ARCH__)
+        const unsigned long long old = atomicCAS(S.keys + at, DF_EMPTY, pair);
+#else
+        const unsigned long long old = S.keys[at];
+        if (old == DF_EMPTY) S.keys[at] = pair;
+#endif
+        if (old == pair) return DF_OLD;
+        if (old != DF_EMPTY) continue;
+#if defined(__CUDA_ARCH__)
+        // one list counter for the whole grid: the lanes that took an entry together take their positions with
+        // one atomic (what cooperative_groups::coalesced_threads() does)
+        const unsigned int act = __activemask(), lane = threadIdx.x & 31u;
+        const int leader = __ffs(act) - 1;
+        unsigned int base = 0;
+        if ((int)lane == leader) base = atomicAdd(S.n, (unsigned int)__popc(act));
+        const unsigned int i = __shfl_sync(act, base, leader) + __popc(act & ((1u << lane) - 1u));
+#else
+        const unsigned int i = (*S.n)++;
+#endif
+        S.list[i] = at;  // i <= mask: every taken entry has one list position
+        if (i < S.limit) return DF_NEW;
+        break;
+    }
+    ctrl->overflow = 1u;
+    return DF_FULL;
+}
+
+// DF: which keys occur in which haystacks of the window, each (haystack, ...) pair once.
+//   lane machines: event(slot) puts (haystack, slot) into P.df_slots; dev_scan.cu's k_df_expand maps each
+//       slot to the keys its event reports (the head record, or for find_overlapping the whole list) and
+//       dedupes again at the key level, where states that share a record or records that share a value meet.
+//   lane per haystack: emit_head / emit_chain put (haystack, key) into P.df_keys directly.
+// `last` drops back-to-back repeats of a slot or key within an item before any atomic; `full` stops the
+// sink once one of its inserts has met the window's overflow.
+struct DfSink {
+    static constexpr int KIND = RK_DF;
+    uint32_t hay = 0, last = 0xffffffffu;
+    bool full = false;
+    DACH_HD void begin(uint32_t item_id) { hay = item_id, last = 0xffffffffu; }
+    DACH_HD void finish(const ScanParams&) {}
+    DACH_HD bool stopped() const { return false; }
+    // as for HistSink: scan_standard routes ROOT's matches through emit_head
+    DACH_HD void emit(const ScanParams&, uint32_t, uint32_t, uint32_t) {}
+    DACH_HD void put(const ScanParams& P, const DfSet& S, uint32_t v) {
+        if (full || v == last) return;
+        last = v;
+        if (df_insert(S, ((unsigned long long)hay << 32) | v, P.ctrl) == DF_FULL) full = true;
+    }
+    DACH_HD void event(const ScanParams& P, uint32_t slot) { put(P, P.df_slots, slot); }
+};
+DACH_HD void emit_head(const ScanParams& P, DfSink& E, uint32_t opos, uint32_t) {
+    E.put(P, P.df_keys, P.df_key_value ? ld_u4(P.outputs + (opos - 1)).x : opos - 1);
+}
+DACH_HD void emit_chain(const ScanParams& P, DfSink& E, uint32_t opos, uint32_t) {
+    while (opos != 0) {
+        const uint4 o = ld_u4(P.outputs + (opos - 1));
+        E.put(P, P.df_keys, P.df_key_value ? o.x : opos - 1);
+        opos = o.z;
+    }
+}
+
 // ---- record access: leading `hot_n` records come from shared memory --------------------
 struct RecView {
     const uint4* glob;
@@ -621,11 +714,17 @@ DACH_HD void scan_standard(const ScanParams& P, const RecView& V, TextWin& T, SI
     if (CHARWISE) root_rec = V.get(D_ROOT);
     if (MODE == M_OVERLAPPING) emit_chain(P, E, root_opos, 0);
     if (MODE == M_NO_SUFFIX && root_opos) {
-        if constexpr (SINK::KIND == RK_HIST) {
+        if constexpr (SINK::KIND == RK_HIST || SINK::KIND == RK_DF) {
             emit_head(P, E, root_opos, 0);
         } else {
             const uint4 o = ld_u4(P.outputs + (root_opos - 1));
             E.emit(P, 0, 0, o.x);  // length 0, end 0 (iter.rs:210-214)
+        }
+    }
+    if constexpr (SINK::KIND == RK_DF) {
+        if (MODE == M_FIND && root_opos) {  // ROOT's record at every boundary, and there is at least one
+            emit_head(P, E, root_opos, 0);
+            return;
         }
     }
     if constexpr (SINK::KIND == RK_HIST) {
@@ -2210,19 +2309,25 @@ struct StdMachine3 {
 //          answer and the item is done; otherwise the queue is emptied and the lane goes on.
 //   HIST   adds 1 per reportable event to the event's slot (HistSink::event): no output list is read
 //          here; dev_scan.cu's post-passes turn slot counts into output-record counts.
+//   DF     puts (haystack, slot) of every reportable event into the window's pair set (DfSink::event),
+//          the haystack of a segment being item_hay[item]; k_df_expand maps slots to keys after the scan.
 // MODE is the machine's iterator: FIRST of a Standard automaton always runs the find_overlapping
 // machine, whose first event is the first event of all three Standard iterators.
 // =============================================================================================
 template <class M, int MODE, int RK>
 struct SinkOps {
-    using Sink = typename std::conditional<RK == RK_COUNT, CountSink,
-                                           typename std::conditional<RK == RK_FIRST, FirstSink, HistSink>::type>::type;
+    using Sink = typename std::conditional<
+        RK == RK_COUNT, CountSink,
+        typename std::conditional<RK == RK_FIRST, FirstSink, typename std::conditional<RK == RK_HIST, HistSink, DfSink>::type>::type>::type;
 
     template <class LANE>
     static DACH_HD void begin_item(LANE& L, const ScanParams& P, const StdEnv& Ev, Sink& E, uint64_t item, const uint8_t* emu_lo) {
         Emitter unused;  // the machines only name the item to their sink
         M::begin_item(L, P, Ev, unused, item, emu_lo);
         E.begin((uint32_t)item);
+        if constexpr (RK == RK_DF) {
+            if (P.item_hay) E.hay = P.item_hay[item];  // a segment counts for its haystack
+        }
         if constexpr (RK == RK_FIRST) {
             if (L.qn) {  // ROOT's list at position 0 (an empty pattern): reportable at once
                 E.emit(P, 0, 0, ld_u4(P.outputs + (ld_u32(Ev.opos + (Ev.q[0].opos & QSLOT_MASK)) - 1)).x);
@@ -2247,7 +2352,7 @@ struct SinkOps {
                 }
             }
             L.qn = 0;
-        } else if constexpr (RK == RK_HIST) {
+        } else if constexpr (RK == RK_HIST || RK == RK_DF) {
             for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j) {
                 if (j < L.qn) {
                     const QEntry e = Ev.q[j * Ev.q_stride];

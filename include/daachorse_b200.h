@@ -243,6 +243,35 @@ int dach_dev_hist_batch(dach_dev *dev, int mode, int key, const uint8_t *d_text,
 int dach_hist_batch_host(dach_dev *dev, int mode, int key, const uint8_t *text, const uint64_t *offs,
                          uint64_t n, uint64_t *hist, uint64_t n_hist, uint64_t *total);
 
+/* ---- per-pattern document frequencies ---------------------------------------------------------
+ *
+ * In how many haystacks of a batch each pattern occurs, with no match list: df[k] += the number of
+ * haystacks h for which iterator `mode`, run on h, yields at least one match whose key is k.  Keys are
+ * those of the histogram calls (dach_hist_key); with DACH_KEY_VALUE two patterns of the same value count a
+ * haystack once.  *total = the sum of the increments, i.e. the number of distinct (haystack, key) pairs.
+ * So df[k] <= n, df <= the histogram of the same batch, and df[k] > 0 exactly where the histogram is; a
+ * haystack counts once however many matches of k it has.  Counts are ADDED into the caller's buffer, so
+ * batches A and B leave what one call on A ++ B would (accumulate across batches, all-reduce across GPUs).
+ * Sizes, keys and modes are checked as for dach_dev_hist_batch; offsets are checked before any scan.
+ * On any error return the caller's df is unchanged: the counts are gathered in a buffer of the library
+ * and added into df only after the whole batch has succeeded.  The calls synchronise `stream`.
+ *
+ * The batch is scanned in windows of whole haystacks (the slices of dach_scan_batch_host).  Each window
+ * dedupes its (haystack, state) and (haystack, key) pairs in two hash sets in device memory owned by the
+ * handle; option df_pairs (default 2^24) is the most pairs either set may take in one window, and is
+ * raised to at least max(compact states, output records) so that one haystack always fits.  Each set
+ * takes the next power of two at or above 2 x df_pairs entries of 12 bytes: 768 MiB of device memory
+ * for both at the default, allocated at the handle's first DF call.  A window that would need more is scanned again as two halves (no DACH_OUTPUT_OVERFLOW);
+ * dach_dev_last_df_windows reports the windows and re-scans of the handle's last DF call.
+ * The device form copies the n + 1 offsets to the host once (8 B per haystack).  Jobs, stream chunks and
+ * shard groups have no DF form. */
+int dach_dev_df_batch(dach_dev *dev, int mode, int key, const uint8_t *d_text, const uint64_t *d_offs,
+                      uint64_t n, uint64_t text_bytes, uint64_t *d_df, uint64_t n_df, uint64_t *total,
+                      void *stream);
+int dach_df_batch_host(dach_dev *dev, int mode, int key, const uint8_t *text, const uint64_t *offs,
+                       uint64_t n, uint64_t *df, uint64_t n_df, uint64_t *total);
+int dach_dev_last_df_windows(const dach_dev *dev, uint64_t *windows, uint64_t *rescans);
+
 /* ---- asynchronous scans (jobs) ----------------------------------------------------------
  *
  * dach_dev_scan_batch is one call that synchronises its stream and serialises per handle.  A job is
@@ -326,7 +355,8 @@ uint64_t dach_dev_last_h2d_bytes(const dach_dev *dev);
 uint64_t dach_dev_last_d2h_bytes(const dach_dev *dev);
 /* Tuning knobs: kernel (3 = StdMachine3, the default; 2, 1 = its predecessors; 0 = lane per haystack),
  * hot_entries (records of the hot region staged in shared memory, default 6144), threads, ctas_per_sm, seg_len
- * (segment length for intra-haystack chunking of find_overlapping), l2_hints, slice_mib, ... */
+ * (segment length for intra-haystack chunking of find_overlapping), l2_hints, slice_mib, df_pairs (a memory
+ * bound: the most pairs per window of the DF calls; see dach_dev_df_batch), ... */
 int dach_dev_set_option(dach_dev *dev, const char *name, int64_t value);
 
 /* Human-readable text of the last error on this thread ("" if none). */

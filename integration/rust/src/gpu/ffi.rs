@@ -87,6 +87,14 @@ extern "C" {
                                 hist: *mut u64, n_hist: u64, total: *mut u64) -> i32;
     pub fn dach_dev_hist_batch(dev: *mut DachDev, mode: i32, key: i32, d_text: *const u8, d_offs: *const u64, n: u64,
                                text_bytes: u64, d_hist: *mut u64, n_hist: u64, total: *mut u64, stream: *mut c_void) -> i32;
+    /// Haystacks with at least one match per key, ADDED into df[0..n_df) (keys as for the histogram); *total = the
+    /// distinct (haystack, key) pairs.  On any error df is unchanged.
+    pub fn dach_df_batch_host(dev: *mut DachDev, mode: i32, key: i32, text: *const u8, offs: *const u64, n: u64,
+                              df: *mut u64, n_df: u64, total: *mut u64) -> i32;
+    pub fn dach_dev_df_batch(dev: *mut DachDev, mode: i32, key: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                             text_bytes: u64, d_df: *mut u64, n_df: u64, total: *mut u64, stream: *mut c_void) -> i32;
+    /// Windows and re-scans (windows that overflowed option df_pairs) of the handle's last DF call.
+    pub fn dach_dev_last_df_windows(dev: *const DachDev, windows: *mut u64, rescans: *mut u64) -> i32;
     /// Device-resident buffers.
     pub fn dach_dev_scan_batch(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
                                text_bytes: u64, d_out: *mut DachMatch, out_cap: u64, d_out_offs: *mut u64,

@@ -4,10 +4,12 @@
     python tools/bench_reduce.py --output counts [--config C3|C3-find|C2|C4|C5] [--steps K] [--warmup W]
     python tools/bench_reduce.py --output first  ...
     python tools/bench_reduce.py --output hist [--key value|output] ...
+    python tools/bench_reduce.py --output df [--key value|output] ...
 
-One step = one dach_dev_count_batch / dach_dev_first_batch / dach_dev_hist_batch on the step's batch (the batches,
-automata and seeds of bench.py).  One JSON line, bench.py's fields where they apply:
-  value              bytes offered / device time of the call's pipeline (CUDA events inside the library)
+One step = one dach_dev_count_batch / dach_dev_first_batch / dach_dev_hist_batch / dach_dev_df_batch on the step's
+batch (the batches, automata and seeds of bench.py).  One JSON line, bench.py's fields where they apply:
+  value              bytes offered / device time of the call's pipeline (CUDA events inside the library; df: CUDA events
+                     around whole steps, since a step is many windows)
   roofline           bench.py's definition, on the COUNT / FIRST scan kernel
   e2e                the same batch through dach_count_batch_host / dach_first_batch_host from pinned host text
   parity             per-haystack counts and their total (counts), or first tuples and found flags (first), against
@@ -19,6 +21,10 @@ automata and seeds of bench.py).  One JSON line, bench.py's fields where they ap
                      matches scan (dach_dev_scan_batch) + torch.bincount of the values, and COUNT; the hist parity
                      checks the value-keyed histogram against np.bincount of the oracle sample's values, and the whole
                      step against the full scan bincounted on the device
+  alternatives       (df) in the same run: the document-frequency call, the full matches scan + the haystack index of
+                     every match, torch.unique of the (haystack, key) pairs and a bincount, and the histogram call; the
+                     df parity checks the value-keyed counts against np.unique of the oracle sample's (haystack, value)
+                     pairs, and the whole step against the matches path; windows / rescans of the last call
   launches_per_step  kernels launched per step
 Nothing is written to the tree.
 """
@@ -58,6 +64,16 @@ def hist_parity(got_hist, ref_values, n_hist):
             "total_equal": int(got.sum()) == int(len(ref_values))}
 
 
+def df_parity(got_df, ref_counts, ref_values, n_df):
+    """In-run parity of --output df (value key) on the oracle sample: the counts against a bincount of np.unique of the
+    oracle's (haystack, value) pairs, and their total against the number of those pairs."""
+    hay = np.repeat(np.arange(len(ref_counts), dtype=np.uint64), np.asarray(ref_counts, dtype=np.int64))
+    pairs = np.unique((hay << np.uint64(32)) | np.asarray(ref_values, dtype=np.uint64))
+    ref = np.bincount((pairs & np.uint64(0xffffffff)).astype(np.int64), minlength=n_df).astype(np.uint64)
+    got = np.asarray(got_df).astype(np.uint64)
+    return {"df_equal": bool(len(got) == len(ref) and np.array_equal(got, ref)), "total_equal": int(got.sum()) == int(len(pairs))}
+
+
 def first_from_matches(matches, counts):
     """(first tuples (k, 3) u32, found (k,)) of haystacks whose runs of `matches` have lengths `counts`; all-ones
     where a haystack has none."""
@@ -88,6 +104,8 @@ def run_reduce_output(args, W, pma, batches, dmode, omode, n, hay_len, step_byte
     import torch
 
     setup_s = time.time() - t_setup
+    if args.output == "df":
+        return run_df_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s)
     if args.output == "hist":
         return run_hist_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s)
     counts_t = torch.empty(n, dtype=torch.int64, device=dev)
@@ -339,10 +357,139 @@ def run_hist_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes,
     }
 
 
+def run_df_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s):
+    """--output df: every step is one dach_dev_df_batch on the step's batch, added into one device array.  The same run
+    times the matches path + torch (haystack index per match, torch.unique of (haystack, key), bincount) and the
+    histogram call on the same batches, step by step, by CUDA events around whole steps."""
+    import torch
+
+    vals = pma.outputs()[0]
+    n_df = (int(vals.max()) + 1 if len(vals) else 0) if args.key == "value" else len(vals)
+    df_t = torch.zeros(n_df, dtype=torch.int64, device=dev)
+    hist_t = torch.zeros(n_df, dtype=torch.int64, device=dev)
+    r0 = pma.scan_batch_device(dmode, *batches[0])
+    cap = int(max(r0.matches.shape[0], 1) * 1.25) + 1024
+    del r0
+    out_m = torch.empty((cap, 3), dtype=torch.int32, device=dev)
+    out_o = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    hay_ids = torch.arange(n, device=dev)
+    key_of_value = torch.from_numpy(np.argsort(vals, kind="stable").astype(np.int64)).to(dev)  # new(): record of value v
+
+    def df_step(s):
+        t, o = batches[s % len(batches)]
+        pma.doc_counts_device(dmode, t, o, key=args.key, out=df_t)
+        st = pma.stats()
+        return st["scan_kernel_ms"], st["total_ms"], pma.last_doc_windows()
+
+    def matches_df(t, o):
+        r = pma.scan_batch_device(dmode, t, o, out=out_m, out_offs=out_o)
+        keys = r.matches[:, 2].long()
+        if args.key == "output":
+            keys = key_of_value[keys]
+        hay = torch.repeat_interleave(hay_ids[: o.numel() - 1], torch.diff(r.offsets.long()))
+        return torch.bincount(torch.unique(hay * n_df + keys) % n_df, minlength=n_df)
+
+    def matches_step(s):
+        return matches_df(*batches[s % len(batches)])
+
+    def hist_step(s):
+        t, o = batches[s % len(batches)]
+        pma.pattern_counts_device(dmode, t, o, key=args.key, out=hist_t)
+
+    def timed(fn):
+        for s in range(args.warmup):
+            fn(s)
+        torch.cuda.synchronize()
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+        res = [fn(args.warmup + s) for s in range(args.steps)]
+        ev1.record()
+        torch.cuda.synchronize()
+        return ev0.elapsed_time(ev1) / args.steps, res
+
+    sampler = ClockSampler(dev.index)
+    sampler.start()
+    time.sleep(0.2)
+    n_before = len(sampler.rows)
+    launches1 = pma.stats()["launches"]
+    df_ms, times = timed(df_step)
+    launches2 = pma.stats()["launches"]
+    matches_ms, _ = timed(matches_step)
+    hist_ms, _ = timed(hist_step)
+    time.sleep(0.25)
+    clocks = sampler.stop(skip=n_before)
+    # a step is many windows, each timed inside the library; the step is timed by the events around it
+    k_ms = float(np.mean([t[0] for t in times]))
+    windows = [t[2] for t in times]
+    gbs = lambda ms: step_bytes / (ms * 1e-3) / 1e9  # noqa: E731
+    value = gbs(df_ms)
+    # the whole last step against the matches path of the same batch, and the histogram invariants
+    last_batch = (args.warmup + args.steps - 1) % len(batches)
+    t_last, o_last = batches[last_batch]
+    one = pma.doc_counts_device(dmode, t_last, o_last, key=args.key)
+    step_ok = bool(torch.equal(one, matches_df(t_last, o_last)))
+    h = pma.pattern_counts_device(dmode, t_last, o_last, key=args.key)
+    vs_hist = {"df_le_hist": bool((one <= h).all()), "same_support": bool(torch.equal(one > 0, h > 0)),
+               "df_le_n": bool(int(one.max()) <= n) if n_df else True}
+    total = int(one.sum().item())
+    parity = None
+    if not args.no_cpu:
+        import oracle_api as O
+
+        threads = O.cpu_budget()["threads"]
+        ns = max(1, min(n, int(n * args.parity_frac)))
+        opma = W.oracle()
+        lo = W.batch_ranges()[last_batch][0]
+        ptext, poffs = W.host_batch(lo, lo + ns)
+        ref = opma.scan_batch(omode, ptext, poffs, nthreads=threads, want_matches=True)
+        nv = int(vals.max()) + 1 if len(vals) else 0
+        got = pma.doc_counts_host(dmode, ptext, poffs, key="value")
+        parity = df_parity(got, ref["counts"], ref["matches"]["value"], nv)
+        parity.update({"haystacks_checked": ns, "share_of_batch": ns / n,
+                       "what": "value-keyed document frequencies of the first %d haystacks of the last batch vs np.unique "
+                               "of the oracle's (haystack, value) pairs" % ns})
+    parity = dict(parity or {}, step_equals_matches_path=step_ok, **vs_hist)
+    e2e = None
+    if not args.no_e2e:
+        t0_, o0_ = batches[0]
+        h_text_t = torch.empty(t0_.numel(), dtype=torch.uint8).pin_memory()
+        h_text_t.copy_(t0_)
+        h_text = h_text_t.numpy()
+        h_offs = o0_.cpu().numpy().astype(np.uint64)
+        e2e_ms = []
+        for i in range(1 + args.e2e_steps):
+            t0 = time.perf_counter()
+            pma.doc_counts_host(dmode, h_text, h_offs, key=args.key)
+            if i >= 1:
+                e2e_ms.append((time.perf_counter() - t0) * 1e3)
+        st = pma.stats()
+        e2e = {"value": h_text.size / (np.mean(e2e_ms) * 1e-3) / 1e9, "unit": UNIT, "h2d_bytes_per_step": int(st["h2d_bytes"]),
+               "d2h_bytes_per_step": int(st["d2h_bytes"]), "ms_per_step": float(np.mean(e2e_ms)), "windows": pma.last_doc_windows(),
+               "workload": "the step batch's %d haystacks x %d B through the host entry point: pinned host text -> device -> "
+                           "scan -> %d x 8 B to the host" % (n, hay_len, n_df)}
+        del h_text_t
+    return {
+        "metric": metric_name(W.spec) + ", df (%s key)" % args.key, "output": "df", "key": args.key, "value": value, "unit": UNIT,
+        "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": df_ms,
+        "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
+        "config": {"workload": "%s: %s, %s, %d haystacks x %d B per step, %d batch(es) resident (%.2f GiB)" % (
+                       args.config, W.spec["what"], W.mode_name, n, hay_len, len(batches), resident / 2**30),
+                   "n_patterns": len(W.ps), "hay_len": hay_len, "bytes_per_gpu": step_bytes, "options": args.option,
+                   "setup_s": setup_s, "n_df": n_df},
+        "total": total, "last_window_scan_kernel_ms": k_ms,
+        "windows_per_step": float(np.mean([w[0] for w in windows])), "rescans_per_step": float(np.mean([w[1] for w in windows])),
+        "alternatives": {"unit": UNIT, "what": "CUDA events around %d whole steps each, same batches" % args.steps,
+                         "df": gbs(df_ms), "matches_plus_torch_unique": gbs(matches_ms), "hist": gbs(hist_ms),
+                         "df_ms": df_ms, "matches_plus_torch_unique_ms": matches_ms, "hist_ms": hist_ms},
+        "card": _card(), "parity": parity, "e2e": e2e,
+        "gpu_launches": int(launches2 - launches1), "launches_per_step": (launches2 - launches1) / args.steps, "clocks": clocks,
+    }
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--output", required=True, choices=["counts", "first", "hist"])
-    ap.add_argument("--key", default="value", choices=["value", "output"], help="--output hist: histogram key")
+    ap.add_argument("--output", required=True, choices=["counts", "first", "hist", "df"])
+    ap.add_argument("--key", default="value", choices=["value", "output"], help="--output hist / df: key")
     ap.add_argument("--config", default="C3", choices=sorted(CONFIGS))
     ap.add_argument("--steps", type=int, default=None)
     ap.add_argument("--warmup", type=int, default=3)

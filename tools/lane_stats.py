@@ -14,7 +14,14 @@ counts in shared memory), from tests/emu_hist.
 reports the output-list lengths of find_overlapping events (the matches that end at one position of a haystack come
 from one event, and there are as many as the landed state's list is long): their distribution, and the share of
 events whose list is too long for the length byte StdMachine3 queues with an event (255 or more: the drain reads the
-head record's chain word instead), from the oracle's matches."""
+head record's chain word instead), from the oracle's matches.
+
+    python tools/lane_stats.py --pairs [C3 C3-find C2 C4 ...]
+
+reports what a document-frequency window holds (dach_dev_df_batch, DESIGN.md section 4.9): the distinct (haystack,
+state) pairs the lane machine puts into the first set and the distinct (haystack, key) pairs of the second, per MiB of
+text, on 4 MiB of the workload's own haystacks, from tests/emu_df -- and so how much text one window of option
+df_pairs pairs covers."""
 import ctypes as C
 import os
 import sys
@@ -86,6 +93,30 @@ def event_shares(name, n_hay=256):
     print("   leading slots:  " + "  ".join("< %d %.1f %%" % (k, 100.0 * lead[k] / max(all_, 1)) for k in tops[2:]))
 
 
+def pair_counts(name, mib=4):
+    import emu_df_api as F
+
+    synth, mode = EVENT_CONFIGS[name]
+    cfg = S.config(synth)
+    cw = cfg["variant"] == "charwise"
+    ps = S.make_patterns(cfg)
+    pool, b = S.make_pool(cfg, ps, 16 << 20)
+    kind = 1 if mode == 3 else 0  # C4: LeftmostLongest
+    opma = O.OraclePma.build_packed(ps.blob, ps.offs, charwise=cw, match_kind=kind)
+    hay_len = cfg["hay_len"]
+    n_hay = max(1, (mib << 20) // hay_len)
+    starts = S.window_starts(b, len(pool), n_hay, hay_len)
+    text, offs = S.materialise_host(pool, starts, hay_len)
+    if cw:
+        text = S.pad_to_char_boundary(text.reshape(n_hay, hay_len)).reshape(-1)
+    rc, _, _, info = F.df(opma.serialize(), cw, mode, "output", text, offs, len(ps), df_pairs=1 << 22)
+    assert rc == 0 and info["rescans"] == 0
+    per = len(text) / float(1 << 20)
+    sp, kp = info["slot_pairs"] / per, info["key_pairs"] / per
+    print("== %s: %d patterns, %d haystacks x %d B: per MiB %.0f (haystack, state) pairs, %.0f (haystack, key) pairs; "
+          "the default 2^24 pairs cover %.0f MiB" % (name, len(ps), n_hay, hay_len, sp, kp, (1 << 24) / max(sp, kp, 1)))
+
+
 def list_lengths(name, n_hay=256):
     cfg = S.config(name)
     ps = S.make_patterns(cfg)
@@ -110,6 +141,9 @@ if __name__ == "__main__":
     if sys.argv[1:2] == ["--lists"]:
         for nm in (sys.argv[2:] or ["C3", "C2"]):
             list_lengths(nm)
+    elif sys.argv[1:2] == ["--pairs"]:
+        for nm in (sys.argv[2:] or list(EVENT_CONFIGS)):
+            pair_counts(nm)
     elif sys.argv[1:2] == ["--events"]:
         for nm in (sys.argv[2:] or list(EVENT_CONFIGS)):
             event_shares(nm)

@@ -7,7 +7,7 @@ native, so this is a subset of tests/test_gpu_parity.py that still launches ever
 
 Golden vectors (all iterators x bytewise / charwise), random batches on every kernel option, text buffers at odd
 addresses and with no slack after the last byte (the 8-byte text loads must not touch anything outside), stream
-chunks, event blocks with output lists of 255 and more (k_expand in pool and output order), counts and first matches, per-pattern histograms (both keys, shared-memory counters on and off), asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
+chunks, event blocks with output lists of 255 and more (k_expand in pool and output order), counts and first matches, per-pattern histograms (both keys, shared-memory counters on and off), document frequencies (both keys, the smallest pair table), asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
 import json
 import os
 import sys
@@ -174,6 +174,39 @@ def histograms():
                 n_scans += 1
 
 
+def doc_frequencies():
+    """dach_df_batch_host / dach_dev_df_batch, both keys, on every kernel that serves them, with the default pair table
+    and the smallest (every window overflows until it is small enough); against np.unique of the oracle's (haystack,
+    value) pairs."""
+    global n_scans
+    dev = torch.device("cuda", 0)
+    for cw in (False, True):
+        for kind in (0, 1):
+            pma, opma, text, offs = random_case(60 + 10 * kind + cw, cw, kind)
+            vals = pma.outputs()[0].astype(np.int64)
+            for mode in ([D.LEFTMOST_FIND] if kind else [D.FIND, D.FIND_OVERLAPPING, D.FIND_OVERLAPPING_NO_SUFFIX]):
+                ref = opma.scan_batch(ORC[mode], text, offs, want_matches=True)
+                hay = np.repeat(np.arange(len(offs) - 1, dtype=np.uint64), ref["counts"].astype(np.int64))
+                pairs = np.unique((hay << np.uint64(32)) | ref["matches"]["value"].astype(np.uint64))
+                want = np.bincount((pairs & np.uint64(0xffffffff)).astype(np.int64), minlength=int(vals.max()) + 1).astype(np.uint64)
+                for opts in ({"kernel": 3}, {"kernel": 3, "seg_len": 64}, {"kernel": 3, "df_pairs": 1}, {"kernel": 0, "df_pairs": 1},
+                             {"kernel": 0}):
+                    for k, v in opts.items():
+                        pma.set_option(k, v)
+                    assert np.array_equal(pma.doc_counts_host(mode, text, offs), want), (cw, kind, mode, opts)
+                    assert np.array_equal(pma.doc_counts_host(mode, text, offs, key="output"), want[vals]), (cw, kind, mode, opts)
+                    n_scans += 2
+                    pma.set_option("seg_len", 0)
+                    pma.set_option("df_pairs", 1 << 24)
+                pma.set_option("kernel", 3)
+                pad = 3
+                buf = torch.empty(text.size + pad, dtype=torch.uint8, device=dev)
+                buf[pad:] = torch.from_numpy(text.copy()).to(dev)
+                o = torch.from_numpy(offs.astype(np.int64)).to(dev)
+                assert np.array_equal(pma.doc_counts_device(mode, buf[pad:], o).cpu().numpy().astype(np.uint64), want)
+                n_scans += 1
+
+
 def streams_jobs_groups():
     global n_scans
     dev = torch.device("cuda", 0)
@@ -236,6 +269,7 @@ if __name__ == "__main__":
     event_blocks()
     counts_and_first()
     histograms()
+    doc_frequencies()
     streams_jobs_groups()
     torch.cuda.synchronize()
     print("sanitize.py: %d scans, all equal to the oracle" % n_scans)
