@@ -637,7 +637,8 @@ __global__ void __launch_bounds__(128, 10) k_push(const uint32_t* src, const uns
 // batch's end) only if `last` -- a shard that is not the last one of a gathered result leaves it to its successor
 __global__ void __launch_bounds__(256) k_final_offsets(const unsigned long long* seg_first, const unsigned long long* item_offs,
                                                         uint64_t n, const unsigned long long* base, int last,
-                                                        unsigned long long* out_offs) {
+                                                        unsigned long long* out_offs, const ScanCtrl* ctrl) {
+    if (ctrl->bad_offsets) return;  // the scan is refused: the caller's offsets stay as they were
     const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (h < n || (h == n && last)) out_offs[h] = (base ? *base : 0ull) + item_offs[seg_first ? seg_first[h] : h];
 }
@@ -646,8 +647,9 @@ __global__ void __launch_bounds__(256) k_final_offsets(const unsigned long long*
 // to start and end of every match of that chunk (haystack found by binary search in out_offs).
 __global__ void __launch_bounds__(256) k_add_base(const ScanCtrl* ctrl, const unsigned long long* out_offs, uint64_t n,
                                                    unsigned long long out_cap, const uint32_t* pos_in, uint32_t* out_words) {
+    if (ctrl->overflow || ctrl->bad_offsets) return;  // (refused: out_offs was not written)
     const unsigned long long total = out_offs[n];
-    if (ctrl->overflow || total > out_cap) return;
+    if (total > out_cap) return;
     for (unsigned long long m = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; m < total;
          m += (unsigned long long)gridDim.x * blockDim.x) {
         uint64_t lo = 0, hi = n;  // largest h with out_offs[h] <= m
@@ -809,7 +811,8 @@ __device__ __forceinline__ void add_block_total(unsigned long long v, unsigned l
 }
 
 __global__ void __launch_bounds__(256) k_count_hay(const unsigned long long* seg_first, const unsigned long long* item_count, uint64_t n,
-                                                    unsigned long long* counts, unsigned long long* total) {
+                                                    unsigned long long* counts, unsigned long long* total, const ScanCtrl* ctrl) {
+    if (ctrl->bad_offsets) return;  // the call is refused: the caller's counts stay as they were
     const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long v = 0;
     if (h < n) {
@@ -821,7 +824,9 @@ __global__ void __launch_bounds__(256) k_count_hay(const unsigned long long* seg
 }
 
 __global__ void __launch_bounds__(256) k_first_hay(const unsigned long long* seg_first, const uint4* item_first, uint64_t n,
-                                                    uint32_t* first_words, uint8_t* found, unsigned long long* n_found) {
+                                                    uint32_t* first_words, uint8_t* found, unsigned long long* n_found,
+                                                    const ScanCtrl* ctrl) {
+    if (ctrl->bad_offsets) return;  // the call is refused: the caller's first / found stay as they were
     const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long v = 0;
     if (h < n) {
@@ -1643,7 +1648,7 @@ int enqueue_place(dach_dev* d, Workspace& W, dach_match* d_out, uint64_t out_cap
         }
     }
     k_final_offsets<<<(unsigned)((n + 1 + 255) / 256), 256, 0, st>>>(
-        W.job_seg ? static_cast<const unsigned long long*>(W.seg_first.p) : nullptr, item_offs, n, d_base, last ? 1 : 0, offs64);
+        W.job_seg ? static_cast<const unsigned long long*>(W.seg_first.p) : nullptr, item_offs, n, d_base, last ? 1 : 0, offs64, ctrl);
     ++d->launches;
     if (d_pos_in && n) {
         k_add_base<<<gather_grid, 256, 0, st>>>(ctrl, offs64, n, out_cap, d_pos_in, reinterpret_cast<uint32_t*>(d_out));
@@ -2050,9 +2055,9 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             d->launches += machine ? 3 : 2;
             if (!cuda_ok(cudaMemsetAsync(d->df_n.p, 0, 8, st), "memset pair counts")) return DACH_CUDA_ERROR;
         } else if (rk == RK_COUNT)
-            k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(d_counts), total);
+            k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(d_counts), total, P.ctrl);
         else
-            k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(d_first), d_found, total);
+            k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(d_first), d_found, total, P.ctrl);
         if (rk == RK_COUNT || rk == RK_FIRST) d->launches += 2;  // the scan and k_count_hay / k_first_hay
         else ++d->launches;                                    // the scan
         if (!cuda_ok(cudaGetLastError(), "kernel launch")) return DACH_CUDA_ERROR;

@@ -1182,8 +1182,9 @@ struct StdMachine {
         L.len = hay_len;
         uint32_t start = 0;
         if (P.item_hay && hay >= P.seg_from) {
-            const uint32_t end = beg + P.seg_len;
-            L.len = end < hay_len ? end : hay_len;
+            // in u64: the last segment of a haystack longer than 2^32 - seg_len would wrap to an end below `start`
+            const uint64_t end = (uint64_t)beg + P.seg_len;
+            if (end < hay_len) L.len = (uint32_t)end;
             start = beg > P.warm ? beg - P.warm : 0;  // warm-up: the state at `beg` only depends on these bytes
         }
         L.pos = start;
@@ -1970,8 +1971,8 @@ struct StdMachine2 {
         L.len = hay_len;
         uint32_t start = 0;
         if (P.item_hay && hay >= P.seg_from) {
-            const uint32_t end = beg + P.seg_len;
-            L.len = end < hay_len ? end : hay_len;
+            const uint64_t end = (uint64_t)beg + P.seg_len;  // in u64, as in StdMachine::begin_item
+            if (end < hay_len) L.len = (uint32_t)end;
             start = beg > P.warm ? beg - P.warm : 0;
         }
         L.pos = start;

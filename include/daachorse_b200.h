@@ -149,8 +149,9 @@ size_t dach_dev_image_bytes(const dach_dev *dev); /* bytes resident in HBM for t
  * in d_out then, and nothing at or past d_out + out_cap is written.  A haystack that yields
  * 2^32 or more matches cannot be placed (per-haystack match indices are u32): the call
  * returns DACH_INVALID_ARGUMENT with the exact *needed and writes no match; count such
- * batches with dach_dev_count_batch / dach_dev_hist_batch.  Stream chunks, the host form and
- * jobs behave the same.  DACH_MATCH_KIND_MISMATCH mirrors the crate's panics.  Charwise
+ * batches with dach_dev_count_batch / dach_dev_hist_batch.  Bad offsets (descending, past
+ * text_bytes, a haystack of 4 GiB or more) are DACH_INVALID_ARGUMENT with d_out and d_out_offs left
+ * as they were.  Stream chunks, the host form and jobs behave the same.  DACH_MATCH_KIND_MISMATCH mirrors the crate's panics.  Charwise
  * haystacks must be valid UTF-8 (as &str guarantees in the crate). */
 int dach_dev_scan_batch(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs,
                         uint64_t n, uint64_t text_bytes, dach_match *d_out, uint64_t out_cap,
@@ -201,6 +202,7 @@ int dach_dev_scan_stream(dach_dev *dev, int mode, const uint8_t *d_text, const u
  *          haystacks with a match.  The scan of a haystack stops at its first match.  For Standard automata
  *          the three Standard modes have the same first match (the head of the first output list reached,
  *          ROOT's empty pattern at position 0 included).
+ * On bad offsets both leave d_counts, d_first and d_found as they were.
  *
  * The host forms copy text and offsets to the device in the slices of dach_scan_batch_host; only the
  * per-haystack results come back (8 B, or 13 B, per haystack; dach_dev_last_h2d_bytes / _d2h_bytes).

@@ -21,6 +21,22 @@ def mixed_width_case(seed):
     return kind, pats, np.frombuffer(b"".join(hays), dtype=np.uint8), offs
 
 
+def seeded_reduce_case(cw, kind):
+    """The seeded batches of the reduction tests (HIST, DF, launch shapes): (patterns, text, offs).  Bytewise: 300
+    patterns over "abcd" and 700 haystacks of up to 3000 bytes over "abcde"; charwise: mixed_width_case(9 + kind)."""
+    rng = np.random.default_rng(80 + 3 * kind + cw)
+    if cw:
+        kind_, pats, text, offs = mixed_width_case(9 + kind)
+        assert kind_ == kind
+        return pats, text, offs
+    pats = [bytes(rng.integers(97, 101, size=int(rng.integers(1, 7))).tolist()) for _ in range(300)]
+    lens = rng.integers(0, 3000, size=700)
+    offs = np.zeros(len(lens) + 1, dtype=np.uint64)
+    offs[1:] = np.cumsum(lens)
+    text = rng.integers(97, 102, size=int(offs[-1])).astype(np.uint8)
+    return pats, text, offs
+
+
 def nul_heavy_case(kind, n_patterns=120000, n_hay=1500, max_len=600):
     """Binary patterns of 3..12 bytes and haystacks drawn mostly from 0x00: with more than ~16k patterns the
     automaton is larger than the default hot region of the compact image, so many states sit in the shifted

@@ -1,9 +1,10 @@
 """Edges of the scan's contract on the CPU emulations of the lane logic (tests/emu, tests/emu_events, tests/emu_reduce,
-tests/emu_hist), against the oracle:
+tests/emu_hist, tests/emu_df), against the oracle:
 
   * the 2^32 address line: StdMachine3 keeps the low 32 bits of the text address as its cursor and adds the carry back
     when it forms an address (Lane3::ap, block_of).  Text mapped across 0x1_0000_0000 puts haystacks, segments and
-    their warm-up on both sides of that line;
+    their warm-up on both sides of that line, for matches, COUNT, FIRST, HIST and DF (both keys, with a pair table so
+    small that windows are scanned again as halves);
   * `needed` past 2^32 matches in one haystack: the per-item match counts are u32.  A count that wraps must not come
     back as a small `needed` with DACH_OUTPUT_OVERFLOW (no capacity would help); the scan is refused and `needed` is
     exact.
@@ -15,10 +16,12 @@ import numpy as np
 import pytest
 
 import emu_api as EA
+import emu_df_api as EF
 import emu_events_api as EV
 import emu_hist_api as EH
 import emu_reduce_api as ER
 import oracle_api as O
+from test_emu_df import doc_freq
 
 INVALID_ARGUMENT, OUTPUT_OVERFLOW = 1, 6
 ORC = {0: O.FIND, 1: O.FIND_OVERLAPPING, 2: O.FIND_OVERLAPPING_NO_SUFFIX, 3: O.LEFTMOST_FIND}
@@ -102,7 +105,7 @@ def test_address_line_in_the_emulations(across_the_line, cw, monkeypatch):
     pats = [p.decode() for p in pats] if cw else pats
     spies = {}
     for mod, fn, arg in ((EA, "emu_scan_batch_wire", 4), (EV, "emu_events_scan_wire", 3),
-                         (ER, "emu_reduce_batch_wire", 5), (EH, "emu_hist_batch_wire", 5)):
+                         (ER, "emu_reduce_batch_wire", 5), (EH, "emu_hist_batch_wire", 5), (EF, "emu_df_batch_wire", 5)):
         spy, seen = _spy(mod, fn, arg)
         monkeypatch.setattr(mod, "_lib", spy)
         spies[mod.__name__] = seen
@@ -110,6 +113,9 @@ def test_address_line_in_the_emulations(across_the_line, cw, monkeypatch):
     for kind in kinds + ((1, 2) if cw else ()):
         opma = O.OraclePma.build(pats, charwise=cw, match_kind=kind)
         wire = opma.serialize()
+        recs = ER.image_outputs(wire, cw)  # DF by output record: the record of each value (the pattern index)
+        rec_of = np.zeros(len(pats), dtype=np.int64)
+        rec_of[recs[:, 0].astype(np.int64)] = np.arange(len(recs))
         modes = (3,) if kind else (0, 1, 2)
         for lo, offs in _line_batches(rng):
             text = buf[lo: lo + int(offs[-1])]
@@ -150,6 +156,14 @@ def test_address_line_in_the_emulations(across_the_line, cw, monkeypatch):
                     assert rc == 0 and total == len(want)
                     assert np.array_equal(h[:nv], np.bincount(want["value"], minlength=nv).astype(np.uint64))
                     assert not h[nv:].any()
+                    for key, k, keys in (("value", nv, want["value"].astype(np.int64)), ("output", len(recs), rec_of[want["value"]])):
+                        ref = doc_freq(np.repeat(np.arange(len(counts)), counts.astype(np.int64)), keys, k)
+                        for pairs in (1, 1 << 16):  # 1: the smallest table, windows re-scanned as halves across the line
+                            rc, got, total, _ = EF.df(wire, cw, mode, key, text, offs, k + 5, kernel=kernel, df_pairs=pairs,
+                                                      out=np.full(k + 5, 7, dtype=np.uint64))
+                            assert rc == 0 and total == int(ref.sum()), (kind, mode, lo, kernel, key, pairs)
+                            assert np.array_equal(got[:k] - np.uint64(7), ref), (kind, mode, lo, kernel, key, pairs)
+                            assert (got[k:] == 7).all(), (kind, mode, lo, kernel, key, pairs, "df written past the key range")
     # every binding handed the kernels' lane logic the mapped text itself, not a copy
     for name, seen in spies.items():
         if name == "emu_events_api" and cw:

@@ -8,7 +8,7 @@ import pytest
 
 import daachorse_b200 as D
 import oracle_api as O
-from cases import mixed_width_case
+from cases import seeded_reduce_case
 from daachorse_b200 import _lib
 from daachorse_b200 import synth as S
 
@@ -65,16 +65,7 @@ def check(pma, mode, text, offs, opma=None):
 @pytest.mark.parametrize("cw", [False, True])
 @pytest.mark.parametrize("kind", [0, 1, 2])
 def test_seeded_batches_and_options(cw, kind):
-    rng = np.random.default_rng(80 + 3 * kind + cw)  # the batches of test_gpu_hist.py
-    if cw:
-        kind_, pats, text, offs = mixed_width_case(9 + kind)
-        assert kind_ == kind
-    else:
-        pats = [bytes(rng.integers(97, 101, size=int(rng.integers(1, 7))).tolist()) for _ in range(300)]
-        lens = rng.integers(0, 3000, size=700)
-        offs = np.zeros(len(lens) + 1, dtype=np.uint64)
-        offs[1:] = np.cumsum(lens)
-        text = rng.integers(97, 102, size=int(offs[-1])).astype(np.uint8)
+    pats, text, offs = seeded_reduce_case(cw, kind)
     pma = builder(cw).new().match_kind(kind).build(pats)
     opma = O.OraclePma.build(pats, charwise=cw, match_kind=kind)
     for mode in ([D.LEFTMOST_FIND] if kind else [D.FIND, D.FIND_OVERLAPPING, D.FIND_OVERLAPPING_NO_SUFFIX]):
