@@ -19,7 +19,7 @@ SYMBOLS = [
     "dach_pma_num_elements", "dach_pma_is_charwise", "dach_pma_max_pattern_len", "dach_pma_num_outputs",
     "dach_pma_outputs", "dach_pma_free",
     "dach_dev_upload", "dach_dev_free", "dach_dev_image_bytes", "dach_dev_scan_batch", "dach_dev_scan_stream",
-    "dach_scan_batch_host", "dach_dev_count_batch", "dach_count_batch_host", "dach_dev_first_batch", "dach_first_batch_host",
+    "dach_dev_count_stream", "dach_dev_first_stream", "dach_dev_hist_stream", "dach_scan_batch_host", "dach_dev_count_batch", "dach_count_batch_host", "dach_dev_first_batch", "dach_first_batch_host",
     "dach_dev_hist_batch", "dach_hist_batch_host", "dach_dev_df_batch", "dach_df_batch_host", "dach_dev_last_df_windows",
     "dach_dev_kernel_launches", "dach_dev_last_scan_kernel_ms",
     "dach_dev_last_total_ms", "dach_dev_last_h2d_bytes", "dach_dev_last_d2h_bytes",
@@ -77,6 +77,12 @@ def load():
     L.dach_dev_scan_stream.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, C.c_uint64, vp, vp, vp, C.c_uint64, vp,
                                        C.POINTER(C.c_uint64), vp]
     L.dach_dev_scan_stream.restype = C.c_int
+    L.dach_dev_count_stream.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, C.c_uint64, vp, vp, C.POINTER(C.c_uint64), vp]
+    L.dach_dev_first_stream.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, C.c_uint64, vp, vp, vp, vp, C.POINTER(C.c_uint64), vp]
+    L.dach_dev_hist_stream.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_uint64, C.c_uint64, vp, vp, C.c_uint64,
+                                       C.POINTER(C.c_uint64), vp]
+    for name in ("dach_dev_count_stream", "dach_dev_first_stream", "dach_dev_hist_stream"):
+        getattr(L, name).restype = C.c_int
     L.dach_scan_batch_host.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, vp, C.c_uint64, vp,
                                        C.POINTER(C.c_uint64)]
     L.dach_scan_batch_host.restype = C.c_int

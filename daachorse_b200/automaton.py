@@ -372,6 +372,76 @@ class _Automaton:
             _check(rc)
             return BatchResult(out[: need.value], out_offs)
 
+    # -- stream chunks without a match list -------------------------------------------------------
+    # ``state`` is read and updated in place exactly as ``scan_stream_device`` does it, so calls of every kind may
+    # take turns on one stream.  Nothing can overflow: one call per round, no copy of the state.
+    def _stream_args(self, mode, text):
+        import torch
+
+        self._assert_mode(mode)
+        dev = text.device.index if text.device.index is not None else torch.cuda.current_device()
+        return dev, self.device_handle(dev)
+
+    @staticmethod
+    def _stream_ptr(stream, text):
+        import torch
+
+        return C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
+
+    def count_stream_device(self, mode, text, offs, state, out=None, stream=None):
+        """Matches per chunk of ``scan_stream_device`` without the matches: an int64 CUDA tensor of n counts
+        (``out``: optional preallocated one), ``state`` advanced in place."""
+        import torch
+
+        dev, d = self._stream_args(mode, text)
+        n = offs.numel() - 1
+        if out is None and n >= 0:
+            out = torch.empty(n, dtype=torch.int64, device=text.device)
+        _check_device_batch(text, offs, dev, state=state, counts=out)
+        total = C.c_uint64()
+        _check(_lib.load().dach_dev_count_stream(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
+                                                 C.c_void_p(state.data_ptr()), C.c_void_p(out.data_ptr()), C.byref(total),
+                                                 self._stream_ptr(stream, text)))
+        return out
+
+    def first_stream_device(self, mode, text, offs, state, pos=None, out=None, found=None, stream=None):
+        """The first match ``scan_stream_device`` reports for each chunk: ``(first, found)`` CUDA tensors as in
+        ``first_batch_device``, positions plus ``pos`` (modulo 2^32; chunk-relative without it), ``state`` advanced
+        in place.  Every chunk is still scanned to its end."""
+        import torch
+
+        dev, d = self._stream_args(mode, text)
+        n = offs.numel() - 1
+        if out is None and n >= 0:
+            out = torch.empty((n, 3), dtype=torch.int32, device=text.device)
+        if found is None and n >= 0:
+            found = torch.empty(n, dtype=torch.bool, device=text.device)
+        _check_device_batch(text, offs, dev, state=state, pos=pos, first=out, found=found)
+        nf = C.c_uint64()
+        _check(_lib.load().dach_dev_first_stream(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
+                                                 C.c_void_p(state.data_ptr()), C.c_void_p(pos.data_ptr()) if pos is not None else None,
+                                                 C.c_void_p(out.data_ptr()), C.c_void_p(found.data_ptr()), C.byref(nf),
+                                                 self._stream_ptr(stream, text)))
+        return out, found
+
+    def pattern_counts_stream_device(self, mode, text, offs, state, key="value", out=None, stream=None):
+        """``pattern_counts_device`` on chunks of streams: the histogram of this round's matches of
+        ``scan_stream_device``, added into ``out`` if given (zeros otherwise), ``state`` advanced in place.  Summed
+        over the rounds it is the histogram of the stepper's matches over the whole streams."""
+        import torch
+
+        dev, d = self._stream_args(mode, text)
+        need = self._hist_len(key)
+        if out is None:
+            out = torch.zeros(need, dtype=torch.int64, device=text.device)
+        _check_device_batch(text, offs, dev, state=state, hist=out, hist_len=need)
+        total = C.c_uint64()
+        _check(_lib.load().dach_dev_hist_stream(d, mode, HIST_KEYS[key], C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()),
+                                                offs.numel() - 1, text.numel(), C.c_void_p(state.data_ptr()),
+                                                C.c_void_p(out.data_ptr()), out.numel(), C.byref(total),
+                                                self._stream_ptr(stream, text)))
+        return out
+
     # -- counts and first matches (no match list) -------------------------------------------------
     def _host_batch_args(self, mode, text, offs):
         self._assert_mode(mode)

@@ -16,7 +16,9 @@
 //     k_scan_machine_rk / k_scan_rk  the same machines / loops with a COUNT, FIRST, HIST or DF sink (dach_dev_count_batch,
 //                               dach_dev_first_batch, dach_dev_hist_batch, dach_dev_df_batch), followed by k_count_hay /
 //                               k_first_hay (per-haystack results), k_hist_heads / k_hist_fold (per-pattern counts) or
-//                               k_df_expand / k_df_add / k_df_clear (document frequencies, window by window)
+//                               k_df_expand / k_df_add / k_df_clear (document frequencies, window by window); on stream
+//                               chunks (dach_dev_count_stream, dach_dev_first_stream, dach_dev_hist_stream) with the
+//                               state carried, FIRST's lanes running to the chunk's end and k_first_stream after them
 //     k_offsets_*               exclusive scan of the per-item match counts
 //     k_blk_index               pool blocks listed in output order (large batches)
 //   phase 2
@@ -69,7 +71,7 @@ template <int RK>
 using SinkOf = typename std::conditional<
     RK == RK_COUNT, CountSink,
     typename std::conditional<
-        RK == RK_FIRST, FirstSink,
+        RK == RK_FIRST || RK == RK_FIRST_STREAM, FirstSink,
         typename std::conditional<RK == RK_HIST, HistSink, typename std::conditional<RK == RK_DF, DfSink, Emitter>::type>::type>::type>::type;
 
 template <bool CHARWISE, int MODE, class SINK>
@@ -842,6 +844,25 @@ __global__ void __launch_bounds__(256) k_first_hay(const unsigned long long* seg
     add_block_total(v, n_found);
 }
 
+// FIRST of stream chunks (one item per chunk, never segments): the item's answer, its start and end in stream
+// coordinates -- plus pos[h], modulo 2^32, as k_add_base does for the matches -- or chunk-relative if pos is nullptr
+__global__ void __launch_bounds__(256) k_first_stream(const uint4* item_first, uint64_t n, const uint32_t* pos, uint32_t* first_words,
+                                                       uint8_t* found, unsigned long long* n_found, const ScanCtrl* ctrl) {
+    if (ctrl->bad_offsets) return;  // the call is refused: the caller's first / found stay as they were
+    const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long v = 0;
+    if (h < n) {
+        const uint4 r = item_first[h];
+        const uint32_t b = (r.w && pos) ? pos[h] : 0u;  // no match: the all-ones sentinel stays as it is
+        first_words[h * 3 + 0] = r.x + b;
+        first_words[h * 3 + 1] = r.y + b;
+        first_words[h * 3 + 2] = r.z;
+        found[h] = r.w ? 1 : 0;
+        v = r.w ? 1 : 0;
+    }
+    add_block_total(v, n_found);
+}
+
 // ---- HIST: per-record counts from per-slot counts, then the caller's keys -------------------------------------------
 // k_hist_heads   (lane machines) slot s counted events of its state: they go to the record that heads the state's
 //                list (opos[s]).  Several slots may share a head.
@@ -1316,6 +1337,19 @@ cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int gri
         case 7: return launch_scan_rk_t<true, M_LEFTMOST, RK>(P, grid, threads, smem, st);
     }
     return cudaErrorInvalidValue;
+}
+
+// FIRST of stream chunks: the caller's iterator (find / find_overlapping) on StdMachine3 or CwMachine
+cudaError_t launch_first_stream(bool cw, int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
+    constexpr int R = RK_FIRST_STREAM;
+    if (cw)
+        return mode == M_FIND ? launch_rk_t<CwMachine<M_FIND>, LaneCw, M_FIND, R, false>(P, grid, threads, smem, st)
+                              : launch_rk_t<CwMachine<M_OVERLAPPING>, LaneCw, M_OVERLAPPING, R, false>(P, grid, threads, smem, st);
+    if (mode == M_FIND)
+        return P.hot_entries ? launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, R, true>(P, grid, threads, smem, st)
+                             : launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, R, false>(P, grid, threads, smem, st);
+    return P.hot_entries ? launch_rk_t<StdMachine3<M_OVERLAPPING>, Lane3, M_OVERLAPPING, R, true>(P, grid, threads, smem, st)
+                         : launch_rk_t<StdMachine3<M_OVERLAPPING>, Lane3, M_OVERLAPPING, R, false>(P, grid, threads, smem, st);
 }
 
 int check_mode(const dach_dev* d, int mode) {
@@ -1942,9 +1976,12 @@ DfSet df_set(dach_dev* d, int i) {
 // into d_hist by `key` unless W.pinned->ctrl.overflow is set once W.ev_placed has completed.  The total (matches, or haystacks with a
 // match) lands in W.pinned->total_rk once W.ev_placed has completed.  No block pool, no offsets, no gather: options
 // kernel = 1, 2, 4 run StdMachine3 here (kernel = 0: the lane-per-haystack kernels).
+// d_state_io (stream chunks, dach_dev_*_stream): haystack i is the next chunk of stream i, resumed in and leaving its
+// state there as in enqueue_scan; FIRST then runs the caller's iterator to each chunk's last byte (RK_FIRST_STREAM)
+// and adds d_pos (or nothing) to its positions.  Stream chunks are never cut into segments.
 int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
                uint64_t text_bytes, const uint64_t* d_offs, uint64_t n, uint64_t* d_counts, dach_match* d_first, uint8_t* d_found,
-               cudaStream_t st, int key = 0, uint64_t* d_hist = nullptr) {
+               cudaStream_t st, int key = 0, uint64_t* d_hist = nullptr, uint32_t* d_state_io = nullptr, const uint32_t* d_pos = nullptr) {
     if (n > 0xfffffff0ull) {
         set_error("too many haystacks in one batch (max 2^32-16)");
         return DACH_INVALID_ARGUMENT;
@@ -1964,14 +2001,20 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         const int free_sms = (int)std::min<int64_t>(std::max<int64_t>(d->opt_reserve_sms, 0), d->sm_count - 1);
         const int grid = (d->sm_count - free_sms) * ctas_per_sm;
         // the first event of a haystack is the same for all three Standard iterators: FIRST runs find_overlapping
-        const int mmode = (rk == RK_FIRST && mode != M_LEFTMOST) ? M_OVERLAPPING : mode;
+        // (not on a stream: the state carried after a find match is not the find_overlapping one)
+        const int mmode = (rk == RK_FIRST && mode != M_LEFTMOST && !d_state_io) ? M_OVERLAPPING : mode;
         const bool v1 = d->opt_kernel >= 1 && d->d_crec && !(mmode == M_FIND && d->root_opos != 0);
         const bool cw_machine = v1 && d->charwise;
         const bool lm_machine = v1 && !d->charwise && mmode == M_LEFTMOST;
         const bool std3 = v1 && !d->charwise && mmode != M_LEFTMOST && d->root_base != 0;
         const bool machine = cw_machine || lm_machine || std3;
-        // segments as in enqueue_scan (no tail-only cutting)
-        bool seg = std3 && (mmode == M_OVERLAPPING || mmode == M_NO_SUFFIX) && d->opt_seg_len >= 0 && d->segmentable;
+        if (d_state_io && !std3 && !cw_machine) {  // as enqueue_scan
+            set_error("stream chunks need a Standard lane machine (find / find_overlapping, at most 2^24 states, bytewise: "
+                      "BASE(ROOT) != 0, no empty pattern for find)");
+            return DACH_INVALID_ARGUMENT;
+        }
+        // segments as in enqueue_scan (no tail-only cutting; a chunk of a stream resumes in a given state: it stays one item)
+        bool seg = std3 && !d_state_io && (mmode == M_OVERLAPPING || mmode == M_NO_SUFFIX) && d->opt_seg_len >= 0 && d->segmentable;
         uint32_t seg_len = 0;
         uint64_t n_items_max = n;
         if (seg) {
@@ -1996,6 +2039,7 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         P.ctrl = static_cast<ScanCtrl*>(W.ctrl.p);
         P.item_count = static_cast<unsigned long long*>(W.items_rk.p);
         P.item_first = static_cast<uint4*>(W.items_rk.p);
+        P.state_io = d_state_io;
         uint32_t hist_k = 0;
         if (rk == RK_HIST) {
             if (machine) hist_k = (uint32_t)std::min<int64_t>(std::max<int64_t>(d->opt_hist_smem, 0), std::min<int64_t>(d->n_cslots, 16384));
@@ -2023,6 +2067,7 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         if (!cuda_ok(rk == RK_COUNT  ? launch_rk<RK_COUNT>(which, d->charwise, mmode, P, grid, t, smem, st)
                      : rk == RK_HIST ? launch_rk<RK_HIST>(which, d->charwise, mmode, P, grid, t, smem, st)
                      : rk == RK_DF   ? launch_rk<RK_DF>(which, d->charwise, mmode, P, grid, t, smem, st)
+                     : d_state_io    ? launch_first_stream(d->charwise, mmode, P, grid, t, smem, st)
                                      : launch_rk<RK_FIRST>(which, d->charwise, mmode, P, grid, t, smem, st),
                      "k_scan launch"))
             return DACH_CUDA_ERROR;
@@ -2056,6 +2101,8 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             if (!cuda_ok(cudaMemsetAsync(d->df_n.p, 0, 8, st), "memset pair counts")) return DACH_CUDA_ERROR;
         } else if (rk == RK_COUNT)
             k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(d_counts), total, P.ctrl);
+        else if (d_state_io)
+            k_first_stream<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(P.item_first, n, d_pos, reinterpret_cast<uint32_t*>(d_first), d_found, total, P.ctrl);
         else
             k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(d_first), d_found, total, P.ctrl);
         if (rk == RK_COUNT || rk == RK_FIRST) d->launches += 2;  // the scan and k_count_hay / k_first_hay
@@ -2544,6 +2591,61 @@ int dach_dev_scan_stream(dach_dev* d, int mode, const uint8_t* d_text, const uin
         return scan_locked(d, d->ws, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, d_out, out_cap, d_out_offs, needed,
                            static_cast<cudaStream_t>(stream), d_state, d_pos);
     });
+}
+
+}  // extern "C"
+
+namespace {
+// COUNT / FIRST / HIST of stream chunks: the mode checks of dach_dev_scan_stream, then one enqueue_rk with the state
+int rk_stream(dach_dev* d, int rk, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+              uint32_t* d_state, const uint32_t* d_pos, uint64_t* d_counts, dach_match* d_first, uint8_t* d_found, uint64_t* d_hist,
+              uint64_t* total, void* stream) {
+    if (mode != DACH_FIND && mode != DACH_FIND_OVERLAPPING) {
+        set_error("stream chunks: mode must be DACH_FIND or DACH_FIND_OVERLAPPING (the crate's two steppers)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    const int rc = check_mode(d, mode);
+    if (rc) return rc;
+    return guarded([&]() -> int {
+        std::lock_guard<std::mutex> lk(d->mu);
+        DeviceGuard g(d->device);
+        if (!g.ok) return DACH_CUDA_ERROR;
+        const int r = enqueue_rk(d, d->ws, rk, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, d_counts, d_first, d_found,
+                                 static_cast<cudaStream_t>(stream), key, d_hist, d_state, d_pos);
+        return r ? r : finish_rk(d, d->ws, total);
+    });
+}
+}  // namespace
+
+extern "C" {
+
+int dach_dev_count_stream(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                          uint32_t* d_state, uint64_t* d_counts, uint64_t* total, void* stream) {
+    if (!d || !d_offs || !d_state || (n && !d_counts)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    return rk_stream(d, RK_COUNT, mode, 0, d_text, d_offs, n, text_bytes, d_state, nullptr, d_counts, nullptr, nullptr, nullptr, total, stream);
+}
+
+int dach_dev_first_stream(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                          uint32_t* d_state, const uint32_t* d_pos, dach_match* d_first, uint8_t* d_found, uint64_t* n_found, void* stream) {
+    if (!d || !d_offs || !d_state || (n && (!d_first || !d_found))) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    return rk_stream(d, RK_FIRST, mode, 0, d_text, d_offs, n, text_bytes, d_state, d_pos, nullptr, d_first, d_found, nullptr, n_found, stream);
+}
+
+int dach_dev_hist_stream(dach_dev* d, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                         uint32_t* d_state, uint64_t* d_hist, uint64_t n_hist, uint64_t* total, void* stream) {
+    if (!d || !d_offs || !d_state || (n_hist && !d_hist)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    const int rc = check_hist(d, key, n_hist);
+    if (rc) return rc;
+    return rk_stream(d, RK_HIST, mode, key, d_text, d_offs, n, text_bytes, d_state, nullptr, nullptr, nullptr, nullptr, d_hist, total, stream);
 }
 
 int dach_scan_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n,

@@ -183,6 +183,9 @@ struct ScanParams {
 // or the distinct (haystack, state / key) pairs of the batch (DfSink).  The lane machines and the
 // lane-per-haystack loops are the same for all five; the sink and, for FIRST, the stop rule differ.
 constexpr int RK_MATCHES = 0, RK_COUNT = 1, RK_FIRST = 2, RK_HIST = 3, RK_DF = 4;
+// FIRST on stream chunks (dach_dev_first_stream): a FirstSink, but the item is scanned to its last byte, because the
+// next chunk resumes in the state after it
+constexpr int RK_FIRST_STREAM = 5;
 
 // L2 eviction policies (64-bit descriptors made once per device by k_make_policies, dev_scan.cu):
 //   [0] automaton image (records, output_pos, outputs, mapper): evict_last -- the scan is latency-bound on
@@ -2312,14 +2315,20 @@ struct StdMachine3 {
 //          here; dev_scan.cu's post-passes turn slot counts into output-record counts.
 //   DF     puts (haystack, slot) of every reportable event into the window's pair set (DfSink::event),
 //          the haystack of a segment being item_hay[item]; k_df_expand maps slots to keys after the scan.
+//   FIRST_STREAM  (stream chunks) keeps the full queue and drains like COUNT: the head of the item's first
+//          event is its answer, and the lane goes on to the chunk's last byte, whose state the next chunk
+//          resumes in.  A chunk is never cut into segments and starts with an empty queue (the incoming
+//          state's list was reported with the previous chunk), so every event is reportable.
 // MODE is the machine's iterator: FIRST of a Standard automaton always runs the find_overlapping
-// machine, whose first event is the first event of all three Standard iterators.
+// machine, whose first event is the first event of all three Standard iterators.  FIRST_STREAM runs the
+// caller's iterator: the state a find stepper carries after a match is not the find_overlapping one.
 // =============================================================================================
 template <class M, int MODE, int RK>
 struct SinkOps {
     using Sink = typename std::conditional<
         RK == RK_COUNT, CountSink,
-        typename std::conditional<RK == RK_FIRST, FirstSink, typename std::conditional<RK == RK_HIST, HistSink, DfSink>::type>::type>::type;
+        typename std::conditional<RK == RK_FIRST || RK == RK_FIRST_STREAM, FirstSink,
+                                  typename std::conditional<RK == RK_HIST, HistSink, DfSink>::type>::type>::type;
 
     template <class LANE>
     static DACH_HD void begin_item(LANE& L, const ScanParams& P, const StdEnv& Ev, Sink& E, uint64_t item, const uint8_t* emu_lo) {
@@ -2358,6 +2367,14 @@ struct SinkOps {
                 if (j < L.qn) {
                     const QEntry e = Ev.q[j * Ev.q_stride];
                     if (e.end >= L.from) E.event(P, e.opos & QSLOT_MASK);  // the entry holds the slot
+                }
+            }
+            L.qn = 0;
+        } else if constexpr (RK == RK_FIRST_STREAM) {
+            for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j) {
+                if (j < L.qn && !E.found) {
+                    const QEntry e = Ev.q[j * Ev.q_stride];
+                    emit_head(P, E, ld_u32(Ev.opos + (e.opos & QSLOT_MASK)), e.end);
                 }
             }
             L.qn = 0;

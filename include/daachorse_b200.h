@@ -188,6 +188,35 @@ int dach_dev_scan_stream(dach_dev *dev, int mode, const uint8_t *d_text, const u
                          dach_match *d_out, uint64_t out_cap, uint64_t *d_out_offs,
                          uint64_t *needed, void *stream);
 
+/* ---- stream chunks without a match list --------------------------------------------------------
+ *
+ * The count, first-match and histogram calls (below) on stream chunks.  d_state is read and written
+ * exactly as dach_dev_scan_stream reads and writes it: after any of these calls it holds, bit for bit,
+ * what dach_dev_scan_stream would leave there on the same chunks and incoming states, so calls of every
+ * kind -- the matches form and the crate's own steppers included -- may alternate on one stream.  The
+ * matches() of the incoming state are not repeated.  Modes, the leftmost refusal and the cases with no
+ * lane machine (DACH_INVALID_ARGUMENT; also option kernel = 0) are those of dach_dev_scan_stream; there is
+ * no DACH_OUTPUT_OVERFLOW.  Bad offsets are DACH_INVALID_ARGUMENT and leave d_state, d_counts, d_first,
+ * d_found and d_hist as they were.  The calls synchronise `stream`.
+ *   count  d_counts[i] (u64, written) = the number of matches chunk i yields, exactly out_offs[i+1] -
+ *          out_offs[i] of dach_dev_scan_stream; *total = their sum.
+ *   first  d_first[i] / d_found[i] = the first match dach_dev_scan_stream reports for chunk i, positions
+ *          plus d_pos[i] (modulo 2^32) or chunk-relative if d_pos is NULL; no match: {0xffffffff x 3} and
+ *          0.  *n_found = the chunks with a match.  The scan still runs to the chunk's last byte (the state
+ *          after it is needed).
+ *   hist   added into d_hist with the keys, sizes and checks of dach_dev_hist_batch: over the rounds of a
+ *          stream the sum is the histogram of the stepper's matches over the whole stream.
+ * Document frequencies have no stream form (a document spanning chunks needs a seen set that outlives
+ * the call). */
+int dach_dev_count_stream(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                          uint64_t text_bytes, uint32_t *d_state, uint64_t *d_counts, uint64_t *total, void *stream);
+int dach_dev_first_stream(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                          uint64_t text_bytes, uint32_t *d_state, const uint32_t *d_pos, dach_match *d_first,
+                          uint8_t *d_found, uint64_t *n_found, void *stream);
+int dach_dev_hist_stream(dach_dev *dev, int mode, int key, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                         uint64_t text_bytes, uint32_t *d_state, uint64_t *d_hist, uint64_t n_hist, uint64_t *total,
+                         void *stream);
+
 /* ---- counts and first matches ----------------------------------------------------------------
  *
  * Two questions that need no match list.  Same batch layout, modes, d_offs checks and errors as
@@ -207,7 +236,8 @@ int dach_dev_scan_stream(dach_dev *dev, int mode, const uint8_t *d_text, const u
  * The host forms copy text and offsets to the device in the slices of dach_scan_batch_host; only the
  * per-haystack results come back (8 B, or 13 B, per haystack; dach_dev_last_h2d_bytes / _d2h_bytes).
  * Option kernel = 1, 2 or 4 runs the default lane machines here (kernel = 3); kernel = 0 the lane-per-haystack
- * kernels.  Stream chunks, jobs and shard groups have no count / first form. */
+ * kernels.  Stream chunks have their own forms (dach_dev_count_stream, dach_dev_first_stream); jobs and shard
+ * groups have no count / first form. */
 int dach_dev_count_batch(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
                          uint64_t text_bytes, uint64_t *d_counts, uint64_t *total, void *stream);
 int dach_count_batch_host(dach_dev *dev, int mode, const uint8_t *text, const uint64_t *offs, uint64_t n,
@@ -234,7 +264,8 @@ int dach_first_batch_host(dach_dev *dev, int mode, const uint8_t *text, const ui
  * The host form uses the slices of dach_scan_batch_host, adds them up on the device and copies
  * n_hist x 8 bytes back once (dach_dev_last_d2h_bytes).  Option hist_smem (default 1024; 0 = off):
  * events of the leading compact states are counted in shared memory per CTA first.  Options kernel and
- * the fallbacks as dach_dev_count_batch.  Stream chunks, jobs and shard groups have no histogram form. */
+ * the fallbacks as dach_dev_count_batch.  Stream chunks have dach_dev_hist_stream; jobs and shard groups have no
+ * histogram form. */
 typedef enum {
     DACH_KEY_OUTPUT = 0,
     DACH_KEY_VALUE = 1

@@ -105,6 +105,18 @@ extern "C" {
     pub fn dach_dev_scan_stream(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
                                 text_bytes: u64, d_state: *mut u32, d_pos: *const u32, d_out: *mut DachMatch,
                                 out_cap: u64, d_out_offs: *mut u64, needed: *mut u64, stream: *mut c_void) -> i32;
+    /// Stream chunks without a match list: d_state read and written exactly as dach_dev_scan_stream does.
+    /// Counts per chunk (written), the first match per chunk (positions + d_pos, or chunk-relative if null), or
+    /// occurrences per key ADDED into d_hist.  No DACH_OUTPUT_OVERFLOW.
+    pub fn dach_dev_count_stream(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                                 text_bytes: u64, d_state: *mut u32, d_counts: *mut u64, total: *mut u64,
+                                 stream: *mut c_void) -> i32;
+    pub fn dach_dev_first_stream(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                                 text_bytes: u64, d_state: *mut u32, d_pos: *const u32, d_first: *mut DachMatch,
+                                 d_found: *mut u8, n_found: *mut u64, stream: *mut c_void) -> i32;
+    pub fn dach_dev_hist_stream(dev: *mut DachDev, mode: i32, key: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                                text_bytes: u64, d_state: *mut u32, d_hist: *mut u64, n_hist: u64, total: *mut u64,
+                                stream: *mut c_void) -> i32;
 
     /// Asynchronous two-phase scans with their own workspace: scan and place only enqueue, wait blocks.
     pub fn dach_job_create(dev: *mut DachDev, out: *mut *mut DachJob) -> i32;

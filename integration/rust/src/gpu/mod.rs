@@ -263,4 +263,42 @@ impl StreamScanner<'_> {
                                         d_state, d_pos, d_out, out_cap, d_out_offs, &mut needed, stream))?;
         Ok(needed)
     }
+
+    /// The number of matches `consume_chunks` would report per chunk, into `d_counts` (n x u64); returns their sum.
+    /// The state advances exactly as there, so the calls may alternate on one stream.
+    /// # Safety
+    /// All pointers are device pointers of the sizes `dach_dev_count_stream` documents.
+    pub unsafe fn count_chunks(&self, d_text: *const u8, d_offs: *const u64, n: u64, text_bytes: u64, d_state: *mut u32,
+                               d_counts: *mut u64, stream: *mut core::ffi::c_void) -> Result<u64, GpuError> {
+        let mut total = 0u64;
+        check(ffi::dach_dev_count_stream(self.pma.dev.dev, ffi::DACH_FIND_OVERLAPPING, d_text, d_offs, n, text_bytes,
+                                         d_state, d_counts, &mut total, stream))?;
+        Ok(total)
+    }
+
+    /// Occurrences per key (`ffi::DACH_KEY_OUTPUT` / `ffi::DACH_KEY_VALUE`) of this round's matches, ADDED into
+    /// `d_hist` (n_hist x u64); returns the matches added.
+    /// # Safety
+    /// All pointers are device pointers of the sizes `dach_dev_hist_stream` documents.
+    pub unsafe fn pattern_counts_chunks(&self, key: i32, d_text: *const u8, d_offs: *const u64, n: u64, text_bytes: u64,
+                                        d_state: *mut u32, d_hist: *mut u64, n_hist: u64,
+                                        stream: *mut core::ffi::c_void) -> Result<u64, GpuError> {
+        let mut total = 0u64;
+        check(ffi::dach_dev_hist_stream(self.pma.dev.dev, ffi::DACH_FIND_OVERLAPPING, key, d_text, d_offs, n, text_bytes,
+                                        d_state, d_hist, n_hist, &mut total, stream))?;
+        Ok(total)
+    }
+
+    /// The first match `consume_chunks` would report per chunk into `d_first` / `d_found` (n each), positions plus
+    /// `d_pos` (or chunk-relative if null); returns the chunks with a match.
+    /// # Safety
+    /// All pointers are device pointers of the sizes `dach_dev_first_stream` documents.
+    pub unsafe fn first_chunks(&self, d_text: *const u8, d_offs: *const u64, n: u64, text_bytes: u64, d_state: *mut u32,
+                               d_pos: *const u32, d_first: *mut ffi::DachMatch, d_found: *mut u8,
+                               stream: *mut core::ffi::c_void) -> Result<u64, GpuError> {
+        let mut n_found = 0u64;
+        check(ffi::dach_dev_first_stream(self.pma.dev.dev, ffi::DACH_FIND_OVERLAPPING, d_text, d_offs, n, text_bytes,
+                                         d_state, d_pos, d_first, d_found, &mut n_found, stream))?;
+        Ok(n_found)
+    }
 }

@@ -5,6 +5,7 @@
     python tools/bench_reduce.py --output first  ...
     python tools/bench_reduce.py --output hist [--key value|output] ...
     python tools/bench_reduce.py --output df [--key value|output] ...
+    python tools/bench_reduce.py --stream --output counts|hist [--key value|output] [--config C2|C3|C3-find] ...
 
 One step = one dach_dev_count_batch / dach_dev_first_batch / dach_dev_hist_batch / dach_dev_df_batch on the step's
 batch (the batches, automata and seeds of bench.py).  One JSON line, bench.py's fields where they apply:
@@ -25,6 +26,10 @@ batch (the batches, automata and seeds of bench.py).  One JSON line, bench.py's 
                      every match, torch.unique of the (haystack, key) pairs and a bincount, and the histogram call; the
                      df parity checks the value-keyed counts against np.unique of the oracle sample's (haystack, value)
                      pairs, and the whole step against the matches path; windows / rescans of the last call
+  alternatives       (--stream) each step is one round: the step's batch is the next chunk of n streams, the state
+                     carried from step to step.  GB/s by CUDA events around whole steps of the stream form
+                     (dach_dev_count_stream / dach_dev_hist_stream) and of scan_stream_device + torch on the same
+                     rounds; parity: counts / histogram and the carried state, stream form vs matches stream
   launches_per_step  kernels launched per step
 Nothing is written to the tree.
 """
@@ -104,6 +109,8 @@ def run_reduce_output(args, W, pma, batches, dmode, omode, n, hay_len, step_byte
     import torch
 
     setup_s = time.time() - t_setup
+    if args.stream:
+        return run_stream_output(args, W, pma, batches, dmode, n, hay_len, step_bytes, resident, dev, setup_s)
     if args.output == "df":
         return run_df_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s)
     if args.output == "hist":
@@ -357,6 +364,95 @@ def run_hist_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes,
     }
 
 
+def run_stream_output(args, W, pma, batches, dmode, n, hay_len, step_bytes, resident, dev, setup_s):
+    """--stream --output counts / hist: every step is one round of n streams -- the step's batch is the next chunk of
+    each -- with the state tensor carried from step to step.  The same run plays the same rounds from the same start
+    through scan_stream_device (stream positions, a preallocated output) and derives what the stream form returns from
+    its matches; both are timed by CUDA events around whole steps.  Parity: per-stream counts summed over all rounds,
+    the accumulated histogram and the carried state, stream form against the matches stream."""
+    import torch
+
+    if dmode not in (0, 1):
+        raise SystemExit("--stream: the config's iterator has no stepper (find_iter / find_overlapping_iter only)")
+    vals = pma.outputs()[0]
+    n_hist = (int(vals.max()) + 1 if len(vals) else 0) if args.key == "value" else len(vals)
+    value_of_record = torch.from_numpy(vals.astype(np.int64)).to(dev)
+    rounds = args.warmup + args.steps
+    pos = [torch.full((n,), (((s * hay_len) + 2**31) % 2**32) - 2**31, dtype=torch.int32, device=dev) for s in range(rounds)]  # u32 bits
+    r0 = pma.scan_batch_device(dmode, *batches[0])
+    cap = int(max(r0.matches.shape[0], 1) * 1.25) + 1024
+    del r0
+    out_m = torch.empty((cap, 3), dtype=torch.int32, device=dev)
+    out_o = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    counts_t = torch.empty(n, dtype=torch.int64, device=dev)
+
+    def play(fn):
+        """all rounds from a fresh state; the timed window covers the last args.steps of them"""
+        state = torch.zeros(n, dtype=torch.int32, device=dev)
+        acc = torch.zeros(n if args.output == "counts" else n_hist, dtype=torch.int64, device=dev)
+        for s in range(args.warmup):
+            fn(s, state, acc)
+        torch.cuda.synchronize()
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+        res = [fn(args.warmup + s, state, acc) for s in range(args.steps)]
+        ev1.record()
+        torch.cuda.synchronize()
+        return ev0.elapsed_time(ev1) / args.steps, res, state, acc
+
+    def stream_step(s, state, acc):
+        t, o = batches[s % len(batches)]
+        if args.output == "counts":
+            acc += pma.count_stream_device(dmode, t, o, state, out=counts_t)
+        else:
+            pma.pattern_counts_stream_device(dmode, t, o, state, key=args.key, out=acc)
+        st = pma.stats()
+        return st["scan_kernel_ms"], st["total_ms"]
+
+    def matches_step(s, state, acc):
+        t, o = batches[s % len(batches)]
+        r = pma.scan_stream_device(dmode, t, o, state, pos[s], out=out_m, out_offs=out_o)
+        if args.output == "counts":
+            acc += torch.diff(r.offsets)
+        else:
+            h = torch.bincount(r.matches[:, 2].long(), minlength=int(vals.max()) + 1 if len(vals) else 0)
+            acc += h if args.key == "value" else h[value_of_record]  # new(): one value per record
+
+    sampler = ClockSampler(dev.index)
+    sampler.start()
+    time.sleep(0.2)
+    n_before = len(sampler.rows)
+    launches1 = pma.stats()["launches"]
+    stream_ms, times, st_a, acc_a = play(stream_step)
+    launches2 = pma.stats()["launches"]
+    matches_ms, _, st_b, acc_b = play(matches_step)
+    time.sleep(0.25)
+    clocks = sampler.stop(skip=n_before)
+    k_ms = float(np.mean([t[0] for t in times]))
+    dev_ms = float(np.mean([t[1] for t in times]))
+    gbs = lambda ms: step_bytes / (ms * 1e-3) / 1e9  # noqa: E731
+    what = "counts" if args.output == "counts" else "hist"
+    parity = {"%s_equal" % what: bool(torch.equal(acc_a, acc_b)), "state_equal": bool(torch.equal(st_a, st_b)),
+              "total": int(acc_a.sum().item()), "rounds": rounds,
+              "what": "stream form vs scan_stream_device over the same %d rounds from state 0: %s and the carried state" % (
+                  rounds, "per-stream counts summed over the rounds" if what == "counts" else "the accumulated histogram")}
+    return {
+        "metric": metric_name(W.spec) + ", stream %s" % (what if what == "counts" else "hist (%s key)" % args.key),
+        "output": args.output, "stream": True, "value": gbs(stream_ms), "unit": UNIT, "n_gpus": 1, "steps": args.steps,
+        "warmup": args.warmup, "ms_per_step": stream_ms, "device_ms_per_step": dev_ms, "scan_kernel_ms": k_ms,
+        "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
+        "config": {"workload": "%s: %s, %s, %d streams, one %d B chunk each per step (the step's batch), %d batch(es) resident "
+                               "(%.2f GiB)" % (args.config, W.spec["what"], W.mode_name, n, hay_len, len(batches), resident / 2**30),
+                   "n_patterns": len(W.ps), "hay_len": hay_len, "bytes_per_gpu": step_bytes, "options": args.option,
+                   "setup_s": setup_s},
+        "alternatives": {"unit": UNIT, "what": "CUDA events around %d whole steps each, same rounds" % args.steps,
+                         "stream_" + what: gbs(stream_ms), "scan_stream_plus_torch": gbs(matches_ms),
+                         "stream_%s_ms" % what: stream_ms, "scan_stream_plus_torch_ms": matches_ms},
+        "card": _card(), "parity": parity,
+        "gpu_launches": int(launches2 - launches1), "launches_per_step": (launches2 - launches1) / rounds, "clocks": clocks,
+    }
+
+
 def run_df_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s):
     """--output df: every step is one dach_dev_df_batch on the step's batch, added into one device array.  The same run
     times the matches path + torch (haystack index per match, torch.unique of (haystack, key), bincount) and the
@@ -489,6 +585,7 @@ def run_df_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, r
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--output", required=True, choices=["counts", "first", "hist", "df"])
+    ap.add_argument("--stream", action="store_true", help="--output counts / hist on stream chunks: one round per step")
     ap.add_argument("--key", default="value", choices=["value", "output"], help="--output hist / df: key")
     ap.add_argument("--config", default="C3", choices=sorted(CONFIGS))
     ap.add_argument("--steps", type=int, default=None)
@@ -505,6 +602,8 @@ def main():
         args.steps = CONFIGS[args.config]["steps"]
     if args.steps < 1:
         ap.error("--steps must be at least 1")
+    if args.stream and args.output not in ("counts", "hist"):
+        ap.error("--stream takes --output counts or hist")
 
     import torch
 

@@ -215,8 +215,9 @@ def streams_jobs_groups():
     o = torch.from_numpy(offs.astype(np.int64)).to(dev)
     n = len(offs) - 1
     whole = pma.scan_batch_device(D.FIND_OVERLAPPING, t, o)
-    # stream chunks: two rounds
-    state = torch.zeros(n, dtype=torch.int32, device=dev)
+    # stream chunks: two rounds, the matches call and the count / first / histogram calls on states of their own
+    state, s_count, s_first, s_hist = (torch.zeros(n, dtype=torch.int32, device=dev) for _ in range(4))
+    hist = torch.zeros(pma._hist_len("value"), dtype=torch.int64, device=dev)
     half = (offs[:-1] + (offs[1:] - offs[:-1]) // 2).astype(np.int64)
     for lo, hi in ((offs[:-1].astype(np.int64), half), (half, offs[1:].astype(np.int64))):
         lens = hi - lo
@@ -224,8 +225,17 @@ def streams_jobs_groups():
         co[1:] = np.cumsum(lens)
         ct = np.concatenate([text[int(a): int(b)] for a, b in zip(lo, hi)]) if co[-1] else np.zeros(0, np.uint8)
         tt = torch.from_numpy(ct.copy()).to(dev) if len(ct) else torch.zeros(16, dtype=torch.uint8, device=dev)[:0]
-        pma.scan_stream_device(D.FIND_OVERLAPPING, tt, torch.from_numpy(co).to(dev), state)
-        n_scans += 1
+        cot = torch.from_numpy(co).to(dev)
+        pos = torch.from_numpy(lo.astype(np.int32)).to(dev)
+        r = pma.scan_stream_device(D.FIND_OVERLAPPING, tt, cot, state, pos)
+        counts = pma.count_stream_device(D.FIND_OVERLAPPING, tt, cot, s_count)
+        first, found = pma.first_stream_device(D.FIND_OVERLAPPING, tt, cot, s_first, pos=pos)
+        pma.pattern_counts_stream_device(D.FIND_OVERLAPPING, tt, cot, s_hist, out=hist)
+        assert torch.equal(counts, r.offsets[1:] - r.offsets[:-1])
+        assert torch.equal(found, counts > 0) and torch.equal(first[found], r.matches[r.offsets[:-1][found]])
+        n_scans += 4
+    for s in (s_count, s_first, s_hist):
+        assert torch.equal(s, state)
     for i in range(0, n, 7):
         assert int(state[i].item()) == opma.state_after(text[int(offs[i]): int(offs[i + 1])].tobytes())
     # jobs on two streams
