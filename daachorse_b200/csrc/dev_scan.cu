@@ -61,6 +61,16 @@ namespace dach {
 constexpr int kMaxThreads = 1024;
 constexpr int kMaxDevices = 64;
 constexpr uint32_t kRootBytes = 1024;  // 256 x u32 at the front of dynamic shared memory
+// Staged hot records (option hot_entries; DESIGN.md section 4.1).  kHotAuto, the default, stages kHotQueued records in the
+// kernels with event queues and fills kDirectSmemBudget in k_scan_direct, which has none.
+constexpr int64_t kHotAuto = -2;
+constexpr int64_t kHotQueued = 6144;
+// H100 splits 256 KiB per SM between shared memory and L1 in steps; past the 196 KiB step the next is 228 KiB, which
+// leaves L1 28 KiB instead of 60 KiB -- too little for the record fetches in flight.  A CTA's dynamic shared memory must
+// stay below the step by the 1 KiB the system reserves per CTA and the kernel's static shared memory (512 B allowed).
+constexpr uint32_t kSmemCarveoutStep = 196 * 1024, kSmemPerSmMax = 228 * 1024;
+constexpr uint32_t kDirectSmemBudget = kSmemCarveoutStep - 1024 - 512;
+constexpr int kDirectCarveoutPct = (int)(100ull * kSmemCarveoutStep / kSmemPerSmMax);  // rounds up to the 196 KiB step
 // DF: pairs per window by default (option df_pairs).  DESIGN.md section 4.9 measures the distinct pairs per MiB of
 // text (tools/lane_stats.py --pairs): at most 84 k (C2), so the largest slice cut_slices makes on the bench workloads
 // (540 MiB of C3 find_iter, 26 k pairs per MiB) fits in one window.  Cost: 2 sets x 2^25 entries x 12 B = 768 MiB.
@@ -277,6 +287,83 @@ __global__ void __launch_bounds__(MAXT, MINB) k_scan_machine(ScanParams P) {
 template <class M, class LANE, int MODE, int RK, bool HOT>
 __global__ void __launch_bounds__(1024, 1) k_scan_machine_rk(ScanParams P) {
     scan_machine<M, SinkOps<M, MODE, RK>, LANE, SinkOf<RK>, HOT>(P);
+}
+
+// ---- StdMachine3's matches path without the queue (DirectOps, scan_lane.cuh) --------------------------------------
+// scan_machine's loop, but the lanes store their events at the landing that makes them.  Dynamic shared memory holds
+// the hot records only.  Service phase: the lanes with a pending event that needs a block take one (one atomic for the
+// warp) and store it, then finished items close and new ones start, as in scan_machine.
+template <int MODE, bool HOT>
+__global__ void __launch_bounds__(1024, 1) k_scan_direct(ScanParams P) {
+    using M = StdMachine3<MODE>;
+    using OPS = DirectOps<MODE>;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    uint4* s_hot = reinterpret_cast<uint4*>(smem_raw);
+    __shared__ __align__(8) uint64_t s_bar;
+    if (HOT) {
+        if (threadIdx.x == 0) mbar_init(&s_bar, 1);
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            const uint32_t hot_bytes = P.hot_entries * 16u;
+            mbar_expect_tx(&s_bar, hot_bytes);
+            for (uint32_t off = 0; off < hot_bytes; off += 32768u)
+                tma_bulk_g2s(reinterpret_cast<unsigned char*>(s_hot) + off, reinterpret_cast<const unsigned char*>(P.crec) + off,
+                             min(32768u, hot_bytes - off), &s_bar);
+        }
+    }
+    const StdEnv Ev{P.crec,  s_hot,   smem_u32(s_hot), HOT ? P.hot_entries : 0u, P.opos_tab, P.text_end, P.text_lo, P.root_base, P.root_opos ? CF_OUT : 0u,
+                    nullptr, 0u,      0u,              P.mapper,                 P.mapper_len, ld_u4(P.crec + D_ROOT)};
+    const unsigned FULL = 0xffffffffu;
+    const unsigned lane = threadIdx.x & 31u;
+    Lane3D L;
+    L.fl = M::IDLE;
+    L.qn = 0;
+    L.E.begin(0);
+    bool exhausted = false;
+    const unsigned long long n_items = P.n_items_dev ? *P.n_items_dev : P.n_items;
+    if (HOT) mbar_wait(&s_bar, 0);
+    for (;;) {
+        // ---- service phase (the warp is converged here) ----
+        const bool want = OPS::need_block(L);
+        const unsigned mb = __ballot_sync(FULL, want);
+        uint32_t blk = 0;
+        if (mb) {
+            const int leader = __ffs(mb) - 1;
+            unsigned int b0 = 0;
+            if ((int)lane == leader) b0 = atomicAdd(&P.ctrl->blk_cursor, (unsigned int)__popc(mb));
+            blk = __shfl_sync(FULL, b0, leader) + __popc(mb & ((1u << lane) - 1u));
+        }
+        if (L.fl & F_ACTIVE) OPS::drain(L, Ev, P, blk);
+        if ((L.fl & (F_ACTIVE | F_DONE)) == (F_ACTIVE | F_DONE)) {
+            L.E.finish(P);
+            M::finish_item(L, P);
+            L.fl = M::IDLE;
+        }
+        const bool need = !(L.fl & F_ACTIVE) && !exhausted;
+        const unsigned m = __ballot_sync(FULL, need);
+        if (m) {
+            const int leader = __ffs(m) - 1;
+            unsigned long long base = 0;
+            if ((int)lane == leader) base = atomicAdd(&P.ctrl->next_item, (unsigned long long)__popc(m));
+            base = __shfl_sync(FULL, base, leader);
+            if (need) {
+                const unsigned long long item = base + __popc(m & ((1u << lane) - 1u));
+                if (item < n_items)
+                    OPS::begin_item(L, P, Ev, item);
+                else
+                    exhausted = true;
+            }
+        }
+        if (!__any_sync(FULL, (L.fl & F_ACTIVE) != 0)) break;
+        // ---- lock-step iterations until some lane needs service ----
+        bool stop = false;
+        while (!stop) {
+            M::text_topup(L, Ev, nullptr);
+#pragma unroll 1
+            for (int k = 0; k < M::TOPUP; ++k) (void)M::step(L, Ev, nullptr);
+            stop = __any_sync(FULL, (L.fl & (F_ACTIVE | F3_STOP)) == (F_ACTIVE | F3_STOP));
+        }
+    }
 }
 
 // ---- StdMachine3, two haystacks per lane ------------------------------------------------------------------
@@ -1083,12 +1170,14 @@ struct dach_dev {
     // ---- options (dach_dev_set_option) ----
     int64_t opt_slice_mib = 64;
     // Records of the hot region staged in shared memory by StdMachine3 (the region is laid out hottest first, so
-    // any prefix is the best set of its size).  Staged records take fetches off L1 and L2, but every KiB of shared
-    // memory is a KiB less L1 for the fetches that still miss.  On H100 (C3 / C2 A/B, DESIGN.md section 4.1) the
-    // scan kernel gains up to 7168 records (112 KiB beside 80 KiB of queues) and falls off a cliff at 8192, where
-    // the carveout leaves L1 too small for the misses in flight; 6144 keeps a margin.  0 = off, -1 = as many as fit
-    // next to the event queues.
-    int64_t opt_hot_entries = 6144;
+    // any prefix is the best set of its size).  Staged records take fetches off L1 and L2 up to the point where the
+    // total of shared memory crosses the 196 KiB carveout step and L1 shrinks (DESIGN.md section 4.1).
+    // kHotAuto: kHotQueued beside the event queues, as many as kDirectSmemBudget holds in k_scan_direct.
+    // 0 = off, -1 = as many as fit (next to the event queues, if any).
+    int64_t opt_hot_entries = kHotAuto;
+    // StdMachine3's matches path: 0 = events stored at their landing (k_scan_direct) when the scan runs one CTA per
+    // SM, 1 = through the per-lane event queue (scan_machine with EventOps)
+    int64_t opt_event_queue = 0;
     // HIST on the lane machines: events of the leading compact slots are counted in shared memory per CTA (4 B
     // each, next to the hot records and the queues) before they reach global memory.  0 = off.
     int64_t opt_hist_smem = 1024;
@@ -1232,6 +1321,37 @@ cudaError_t launch_duo(int mode, const ScanParams& P, int grid, int threads, siz
     if (threads > 768)
         return P.hot_entries ? launch_duo_m<1024, true>(mode, P, grid, threads, smem, st) : launch_duo_m<1024, false>(mode, P, grid, threads, smem, st);
     return P.hot_entries ? launch_duo_m<768, true>(mode, P, grid, threads, smem, st) : launch_duo_m<768, false>(mode, P, grid, threads, smem, st);
+}
+
+template <int MODE, bool HOT>
+cudaError_t launch_direct_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
+    static bool attr_done[kMaxDevices] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
+        cudaError_t e = cudaFuncSetAttribute(k_scan_direct<MODE, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+        // the smallest carveout that holds kDirectSmemBudget: L1 keeps what it has beside the queue kernel
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(k_scan_direct<MODE, HOT>, cudaFuncAttributePreferredSharedMemoryCarveout, kDirectCarveoutPct);
+        if (e != cudaSuccess) return e;
+        if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
+    }
+    k_scan_direct<MODE, HOT><<<grid, threads, smem, st>>>(P);
+    return cudaGetLastError();
+}
+// StdMachine3's matches path without the queue (option event_queue = 0, one CTA per SM)
+cudaError_t launch_direct(int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
+    switch (mode) {
+        case M_FIND:
+            return P.hot_entries ? launch_direct_t<M_FIND, true>(P, grid, threads, smem, st) : launch_direct_t<M_FIND, false>(P, grid, threads, smem, st);
+        case M_NO_SUFFIX:
+            return P.hot_entries ? launch_direct_t<M_NO_SUFFIX, true>(P, grid, threads, smem, st)
+                                 : launch_direct_t<M_NO_SUFFIX, false>(P, grid, threads, smem, st);
+        case M_OVERLAPPING:
+            return P.hot_entries ? launch_direct_t<M_OVERLAPPING, true>(P, grid, threads, smem, st)
+                                 : launch_direct_t<M_OVERLAPPING, false>(P, grid, threads, smem, st);
+    }
+    return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_cw(int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
@@ -1401,8 +1521,9 @@ ScanParams image_params(const dach_dev* d, const uint8_t* d_text, const uint8_t*
     return P;
 }
 
-// dynamic shared memory of the scan kernel: the lane machines' event queues (queue_sets per lane) and, for
-// StdMachine3, the front of the hot region; the lane-per-haystack kernels stage leading wide records
+// dynamic shared memory of the scan kernel: the lane machines' event queues (queue_sets per lane; 0 for
+// k_scan_direct) and, for StdMachine3, the front of the hot region; the lane-per-haystack kernels stage leading wide
+// records
 size_t plan_smem(const dach_dev* d, ScanParams& P, bool v1, bool std3, int threads, int ctas_per_sm, int queue_sets,
                  uint32_t hist_smem = 0) {
     const size_t smem_budget = std::min<size_t>(d->smem_optin, 226 * 1024) / ctas_per_sm - (ctas_per_sm > 1 ? 1024 : 0);
@@ -1414,7 +1535,8 @@ size_t plan_smem(const dach_dev* d, ScanParams& P, bool v1, bool std3, int threa
         uint64_t want = 0;
         if (std3 && d->opt_hot_entries != 0 && smem_budget > queues + 512) {
             want = std::min<uint64_t>(d->hot_slots, (smem_budget - queues - 512) / 16);
-            if (d->opt_hot_entries > 0) want = std::min<uint64_t>(want, (uint64_t)d->opt_hot_entries);
+            const int64_t hot = d->opt_hot_entries != kHotAuto ? d->opt_hot_entries : queue_sets ? kHotQueued : kDirectSmemBudget / 16;
+            if (hot > 0) want = std::min<uint64_t>(want, (uint64_t)hot);
             want &= ~uint64_t(255);
         }
         smem = (size_t)want * 16 + queues;
@@ -1500,7 +1622,9 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     const bool std2 = v1 && !d->charwise && mode != M_LEFTMOST && d->opt_kernel >= 2 && d->root_base != 0;
     const bool std3 = std2 && d->opt_kernel >= 3;
     const bool duo = std3 && d->opt_kernel >= 4 && ctas_per_sm == 1;
-    const bool events = std3 && !duo;  // StdMachine3's matches path stores events (k_scan_machine)
+    const bool events = std3 && !duo;  // StdMachine3's matches path stores events (k_scan_machine / k_scan_direct)
+    // ... at their landing, without the queue: one CTA per SM, whose shared memory the staged records fill
+    const bool direct = events && ctas_per_sm == 1 && d->opt_event_queue == 0;
 
     if (d_state_io && !std2 && !cw_machine) {
         set_error("stream chunks need a Standard lane machine (find / find_overlapping, at most 2^24 states, bytewise: "
@@ -1564,7 +1688,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     P.pool_blocks = pool_blocks;
     P.ctrl = static_cast<ScanCtrl*>(W.ctrl.p);
     P.state_io = d_state_io;
-    const size_t smem = plan_smem(d, P, v1, std3, threads, ctas_per_sm, duo ? 2 : 1);
+    const size_t smem = plan_smem(d, P, v1, std3, threads, ctas_per_sm, duo ? 2 : direct ? 0 : 1);
 
     unsigned long long* tiles = static_cast<unsigned long long*>(W.tiles.p);
     unsigned long long* item_offs = static_cast<unsigned long long*>(W.item_offs.p);
@@ -1579,7 +1703,8 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     if (!cuda_ok(cw_machine   ? launch_cw(mode, P, grid, std::min(threads, 1024), smem, st)
                  : lm_machine ? launch_lm(P, grid, std::min(threads, 1024), smem, st)
                  : duo        ? launch_duo(mode, P, grid, threads, smem, st)
-                 : v1         ? launch_std(std3 ? 3 : std2 ? 2 : 1, mode, P, grid, threads, smem, st,
+                 : direct     ? launch_direct(mode, P, grid, threads, smem, st)
+                 : v1        ? launch_std(std3 ? 3 : std2 ? 2 : 1, mode, P, grid, threads, smem, st,
                                            ctas_per_sm >= 2 && threads <= 768 && grid % 2 == 0)
                               : launch_scan(d->charwise, mode, P, grid, threads, smem, st),
                  "k_scan launch"))
@@ -3142,6 +3267,8 @@ int dach_dev_set_option(dach_dev* d, const char* name, int64_t value) {
         d->opt_smem_pad_kib = value;
     else if (k == "hot_entries")
         d->opt_hot_entries = value;
+    else if (k == "event_queue")
+        d->opt_event_queue = value;
     else if (k == "hist_smem")
         d->opt_hist_smem = value;
     else if (k == "df_pairs")

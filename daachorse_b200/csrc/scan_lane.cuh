@@ -2053,6 +2053,16 @@ struct Lane3 {
     uint32_t from;            // drain: only events with end >= from are reported (segment start + 1, or 0)
 };
 
+// The direct matches path (DirectOps, k_scan_direct): no queue.  The lane carries its item's event sink and stores an
+// event into its current block at the landing that makes it; an event that cannot go there (no block with room, or a
+// list length that needs the chain word) waits in (pend_end, pend_slot) for the service phase.
+constexpr uint32_t F3_PEND = 0x40u;   // an event is pending
+constexpr uint32_t F3_CARRY = 0x80u;  // the item's u32 match count wrapped since the last service phase
+struct Lane3D : Lane3 {
+    EventSink E;
+    uint32_t pend_end, pend_slot;
+};
+
 // 8 text bytes at the 8-aligned address q; bytes outside [text_lo, text_end) read as 0 and are never touched
 DACH_HD uint2 ld_text8_safe(const uint8_t* q, const uint8_t* text_lo, const uint8_t* text_end) {
     uint2 w;
@@ -2130,8 +2140,8 @@ struct StdMachine3 {
         L.addr = D_ROOT;
     }
 
-    // the byte is consumed; the lane sits in the state whose record it just adopted
-    static DACH_HD void land(Lane3& L, const StdEnv& Ev) {
+    // the byte under the cursor is consumed: move the text window, note the end of the item
+    static DACH_HD void consume(Lane3& L) {
         ++L.ap;
         L.w0 = (L.w0 >> 8) | (L.w1 << 24);
         L.w1 >>= 8;
@@ -2141,6 +2151,11 @@ struct StdMachine3 {
             L.fl |= F_NEED_NW;
         }
         if (L.ap == L.ap_end) L.fl |= F_DONE | F3_STOP;
+    }
+
+    // the byte is consumed; the lane sits in the state whose record it just adopted
+    static DACH_HD void land(Lane3& L, const StdEnv& Ev) {
+        consume(L);
         if (L.nf & CF_OUT) {
             DACH_STAT(pushes);
             QEntry e;  // one 8-byte store: (end, slot | list length << 24); output_pos is looked up after the scan
@@ -2149,6 +2164,33 @@ struct StdMachine3 {
             Ev.q[L.qn * Ev.q_stride] = e;
             if (++L.qn == (uint32_t)LANE_Q) L.fl |= F3_STOP;
             if (MODE == M_FIND) to_root(L, Ev);  // every next() restarts at ROOT (src/bytewise/iter.rs:87)
+        }
+    }
+    // the direct matches path: the event goes straight into the lane's block (the same 8 bytes the queue held), or
+    // waits for the service phase.  A warm-up event (end < from) is dropped here.  A saturated length byte always
+    // waits: its list length is the head record's chain word, a dependent load the loop never makes.
+    static DACH_HD void land(Lane3D& L, const StdEnv& Ev) {
+        consume(L);
+        if (L.nf & CF_OUT) {
+            DACH_STAT(pushes);
+            const uint32_t end = L.ap - L.hay_lo;
+            if (end >= L.from) {
+                const uint32_t slot = MODE == M_OVERLAPPING ? L.addr | (L.r2 << 24) : L.addr;
+                const uint32_t len = MODE == M_OVERLAPPING ? L.r2 & 0xffu : 1u;
+                if (L.E.fill < BLK_EVENTS && len != QLEN_ESCAPE) {
+                    if (L.E.blk) st_stream_u2(L.E.blk + BLK_HDR_WORDS + 2 * L.E.fill, end, slot);
+                    ++L.E.fill;
+                    ++L.E.nev;
+                    const uint32_t c = L.E.count + len;
+                    if (c < L.E.count) L.fl |= F3_CARRY;
+                    L.E.count = c;
+                } else {
+                    L.pend_end = end;
+                    L.pend_slot = slot;
+                    L.fl |= F3_PEND | F3_STOP;
+                }
+            }
+            if (MODE == M_FIND) to_root(L, Ev);
         }
     }
 
@@ -2162,7 +2204,9 @@ struct StdMachine3 {
         const uint32_t a = ((own ? L.r0 : L.r2) >> 8) ^ c;  // its child, or the failure state's
         return (L.fl & F3_STOP) ? 0u : a;
     }
-    static DACH_HD void resolve(Lane3& L, const StdEnv& Ev, const uint4& x, uint32_t a, uint32_t own) {
+    // LANE: Lane3 (events queued) or Lane3D (events stored at the landing); only land() tells them apart
+    template <class LANE>
+    static DACH_HD void resolve(LANE& L, const StdEnv& Ev, const uint4& x, uint32_t a, uint32_t own) {
         if (L.fl & (F3_STOP | F3_LEARN)) {  // one test keeps both rare cases out of the common path
             if (L.fl & F3_STOP) return;
             // x is the failure state's record (fetched through the own-child path: r0 held its slot ^ c and the
@@ -2205,7 +2249,8 @@ struct StdMachine3 {
             L.fl |= F3_LEARN;
         }
     }
-    static DACH_HD bool step(Lane3& L, const StdEnv& Ev, const uint8_t* emu_lo = nullptr) {
+    template <class LANE>
+    static DACH_HD bool step(LANE& L, const StdEnv& Ev, const uint8_t* emu_lo = nullptr) {
         (void)emu_lo;
         if (L.fl & F3_STOP) return false;
         uint32_t own;
@@ -2439,6 +2484,57 @@ struct EventOps {
             }
         }
         L.qn = 0;
+        if (!(L.fl & F_DONE)) L.fl &= ~F3_STOP;
+    }
+};
+
+// =============================================================================================
+// The matches path of StdMachine3 without the queue (k_scan_direct, the default for one CTA per SM).
+//
+// The queue above batches stores that need no dependent load: since events are stored as they are, the lane can store
+// each one at the landing that makes it (StdMachine3::land(Lane3D&)).  The shared memory of the queue goes to staged
+// records instead, and a warp stops only when a lane needs a block (its block is full, or it has none yet), meets a
+// saturated list length, or ends its item -- not whenever one lane has queued LANE_Q events.  Blocks are the queue
+// path's: header {item, seq, first}, then the item's events in order, BLK_EVENTS per block.
+// Between two service phases a lane stores at most BLK_EVENTS events of at most 254 matches each, so its u32 count
+// wraps at most once in between: the loop flags the wrap (F3_CARRY) and the phase reports it (count_carry).
+// =============================================================================================
+template <int MODE>
+struct DirectOps {
+    using M = StdMachine3<MODE>;
+
+    static DACH_HD void begin_item(Lane3D& L, const ScanParams& P, const StdEnv& Ev, uint64_t item) {
+        // the machine queues ROOT's list at position 0 (an empty pattern) as the item's first event: here it is given a
+        // queue of one entry, and the entry becomes the pending event
+        QEntry root;
+        StdEnv Ev1 = Ev;
+        Ev1.q = &root;
+        Emitter unused;  // the machine only names the item to its sink
+        M::begin_item(L, P, Ev1, unused, item, nullptr);
+        L.E.begin((uint32_t)item);
+        if (L.qn) {
+            L.pend_end = root.end;
+            L.pend_slot = root.opos;
+            L.fl |= F3_PEND | F3_STOP;
+            L.qn = 0;
+        }
+    }
+    static DACH_HD bool need_block(const Lane3D& L) { return (L.fl & F3_PEND) && L.E.fill == BLK_EVENTS; }
+
+    // blk: the pool block this lane was given this phase (used only if need_block() said so)
+    static DACH_HD void drain(Lane3D& L, const StdEnv& Ev, const ScanParams& P, uint32_t blk) {
+        EventSink& E = L.E;
+        if (L.fl & F3_PEND) {
+            if (E.fill == BLK_EVENTS) E.open(P, blk);
+            if (E.blk) st_stream_u2(E.blk + BLK_HDR_WORDS + 2 * E.fill, L.pend_end, L.pend_slot);
+            ++E.fill;
+            ++E.nev;
+            const uint32_t c = E.count + (MODE == M_OVERLAPPING ? qentry_len(P, Ev.opos, L.pend_slot) : 1u);
+            if (c < E.count) count_carry(P);
+            E.count = c;
+        }
+        if (L.fl & F3_CARRY) count_carry(P);
+        L.fl &= ~(F3_PEND | F3_CARRY);
         if (!(L.fl & F_DONE)) L.fl &= ~F3_STOP;
     }
 };

@@ -387,7 +387,10 @@ double dach_dev_last_total_ms(const dach_dev *dev);
 uint64_t dach_dev_last_h2d_bytes(const dach_dev *dev);
 uint64_t dach_dev_last_d2h_bytes(const dach_dev *dev);
 /* Tuning knobs: kernel (3 = StdMachine3, the default; 2, 1 = its predecessors; 0 = lane per haystack),
- * hot_entries (records of the hot region staged in shared memory, default 6144), threads, ctas_per_sm, seg_len
+ * hot_entries (records of the hot region staged in shared memory; the default -2 stages 6144 beside the event
+ * queues and fills the shared memory below the 196 KiB carveout step in the matches scan without them),
+ * event_queue (matches of StdMachine3: 0 = each event stored at the landing that makes it, the default with one
+ * CTA per SM; 1 = through a per-lane shared-memory queue), threads, ctas_per_sm, seg_len
  * (segment length for intra-haystack chunking of find_overlapping), l2_hints, slice_mib, df_pairs (a memory
  * bound: the most pairs per window of the DF calls; see dach_dev_df_batch), ... */
 int dach_dev_set_option(dach_dev *dev, const char *name, int64_t value);

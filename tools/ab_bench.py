@@ -42,7 +42,7 @@ out = torch.empty((r.matches.shape[0] + 1024, 3), dtype=torch.int32, device="cud
 oo = torch.empty(offs_t.numel(), dtype=torch.int64, device="cuda")
 base_sum = int(r.matches.to(torch.int64).sum().item())
 nb = text_t.numel()
-DEFAULTS = {"kernel": 3, "hot_entries": 6144, "threads": 1024, "ctas_per_sm": 1, "l2_hints": 2, "gather_ordered": 1}
+DEFAULTS = {"kernel": 3, "hot_entries": -2, "event_queue": 0, "threads": 1024, "ctas_per_sm": 1, "l2_hints": 2, "gather_ordered": 1}
 for s in (a.sets or ["kernel=3"]):
     opts = dict(DEFAULTS)
     for kv in s.split(","):

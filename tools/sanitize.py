@@ -7,7 +7,8 @@ native, so this is a subset of tests/test_gpu_parity.py that still launches ever
 
 Golden vectors (all iterators x bytewise / charwise), random batches on every kernel option, text buffers at odd
 addresses and with no slack after the last byte (the 8-byte text loads must not touch anything outside), stream
-chunks, event blocks with output lists of 255 and more (k_expand in pool and output order), counts and first matches, per-pattern histograms (both keys, shared-memory counters on and off), document frequencies (both keys, the smallest pair table), asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
+chunks, event blocks with output lists of 255 and more (stored at the landing and through the event queue; k_expand in
+pool and output order), counts and first matches, per-pattern histograms (both keys, shared-memory counters on and off), document frequencies (both keys, the smallest pair table), asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
 import json
 import os
 import sys
@@ -68,8 +69,8 @@ def random_batches():
             pma, opma, text, offs = random_case(10 * kind + cw, cw, kind)
             for mode in ([D.LEFTMOST_FIND] if kind else [D.FIND, D.FIND_OVERLAPPING, D.FIND_OVERLAPPING_NO_SUFFIX]):
                 ref = opma.scan_batch(ORC[mode], text, offs, want_matches=True)
-                for opts in ({"kernel": 3}, {"kernel": 4}, {"kernel": 3, "hot_entries": 512}, {"kernel": 2}, {"kernel": 1}, {"kernel": 0},
-                             {"kernel": 3, "seg_len": 64}, {"kernel": 4, "threads": 256}):
+                for opts in ({"kernel": 3}, {"kernel": 3, "event_queue": 1}, {"kernel": 4}, {"kernel": 3, "hot_entries": 512}, {"kernel": 2},
+                             {"kernel": 1}, {"kernel": 0}, {"kernel": 3, "seg_len": 64}, {"kernel": 4, "threads": 256}):
                     for k, v in opts.items():
                         pma.set_option(k, v)
                     r = pma.scan_batch_host(mode, text, offs)
@@ -78,6 +79,7 @@ def random_batches():
                     pma.set_option("seg_len", 0)
                     pma.set_option("hot_entries", 0)
                     pma.set_option("threads", 1024)
+                    pma.set_option("event_queue", 0)
                 pma.set_option("kernel", 3)
                 # device-resident text at an odd address, the last haystack ending exactly at the end of the allocation
                 pad = 3
@@ -101,13 +103,15 @@ def event_blocks():
     pma, opma = D.DoubleArrayAhoCorasick.new(pats), O.OraclePma.build(pats)
     for mode in (D.FIND, D.FIND_OVERLAPPING, D.FIND_OVERLAPPING_NO_SUFFIX):
         ref = opma.scan_batch(ORC[mode], text, offs, want_matches=True)
-        for opts in ({"gather_ordered": 0}, {"gather_ordered": 2}, {"gather_ordered": 2, "seg_len": 64}):
+        for opts in ({"gather_ordered": 0}, {"gather_ordered": 2}, {"gather_ordered": 2, "seg_len": 64}, {"event_queue": 1},
+                     {"event_queue": 1, "seg_len": 64}):
             for k, v in opts.items():
                 pma.set_option(k, v)
             r = pma.scan_batch_host(mode, text, offs)
             assert r.matches.tobytes() == ref["matches"].tobytes(), (mode, opts)
             n_scans += 1
             pma.set_option("seg_len", 0)
+            pma.set_option("event_queue", 0)
         pma.set_option("gather_ordered", 1)
 
 
