@@ -262,6 +262,19 @@ int build_image(const dach_pma* p, HostImage* img) {
         const uint32_t par = p->outputs[i].parent;
         img->outputs[i * 4 + 3] = 1u + (par ? img->outputs[(size_t)(par - 1) * 4 + 3] : 0u);
     }
+    // two-entry lists (k_expand_desc): the record and its parent in one 16-byte entry, the list length's class in
+    // the top two bits of the parent's length.  Only if no pattern length reaches those bits.
+    img->pairs.clear();
+    if (img->max_pattern_len < PAIR_LEN_MASK) {
+        img->pairs.resize(p->outputs.size() * 4);
+        for (size_t i = 0; i < p->outputs.size(); ++i) {
+            const uint32_t par = p->outputs[i].parent, len = img->outputs[i * 4 + 3];
+            img->pairs[i * 4 + 0] = p->outputs[i].value;
+            img->pairs[i * 4 + 1] = p->outputs[i].length;
+            img->pairs[i * 4 + 2] = par ? p->outputs[par - 1].value : 0u;
+            img->pairs[i * 4 + 3] = (par ? p->outputs[par - 1].length : 0u) | (len < 3u ? len : 3u) << PAIR_CLASS_SHIFT;
+        }
+    }
 
     img->rec.resize(n * 4);
     if (!p->charwise) {

@@ -8,6 +8,12 @@
 
 namespace dach {
 
+// Two-entry output lists (HostImage::pairs, read by k_expand_desc): per output record {value, length, parent's value,
+// parent's length | class << 30}, class = the length of the list that starts at the record, saturated at 3.  Class 1
+// leaves the parent's fields 0; class 3 lists are walked through the outputs from the head.
+constexpr uint32_t PAIR_CLASS_SHIFT = 30;
+constexpr uint32_t PAIR_LEN_MASK = (1u << PAIR_CLASS_SHIFT) - 1u;
+
 struct HostImage {
     bool charwise = false;
     uint8_t match_kind = 0;
@@ -16,6 +22,7 @@ struct HostImage {
     uint32_t max_pattern_len = 0;
     std::vector<uint32_t> rec;         // 4 words per slot
     std::vector<uint32_t> outputs;     // 4 words per output
+    std::vector<uint32_t> pairs;       // 4 words per output (PAIR_* in scan_lane.cuh), empty if a pattern length is >= 2^30
     std::vector<uint32_t> root_table;  // 256 words (bytewise)
     std::vector<uint32_t> crec;        // compact records, 4 words per slot (bytewise Standard, <= 2^24 slots)
     std::vector<uint32_t> opos_tab;    // output_pos per slot (with crec)

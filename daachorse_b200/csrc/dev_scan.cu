@@ -686,6 +686,101 @@ __global__ void __launch_bounds__(256) k_expand(const uint32_t* pool, const Scan
     }
 }
 
+// Block descriptors of the ordered event placement (k_expand_desc): desc[j] = {pool block, its events, u64 index of its
+// first match in the batch} for the j-th block in output order.  k_blk_index's walk; the header, ev_counts and
+// item_offs are looked up here, on the scan stream, so that the placement's chain of dependent loads starts at the
+// block's events.
+__global__ void __launch_bounds__(256) k_blk_desc(const uint32_t* pool, const ScanCtrl* ctrl, uint32_t pool_blocks,
+                                                   const unsigned long long* blk_first, const uint32_t* ev_counts,
+                                                   const unsigned long long* item_offs, uint4* desc) {
+    if (ctrl->overflow) return;
+    const uint32_t used = min(ctrl->blk_cursor, pool_blocks);
+    for (uint64_t b = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; b < used; b += (uint64_t)gridDim.x * blockDim.x) {
+        const uint4 h = *reinterpret_cast<const uint4*>(pool + b * BLK_WORDS);  // {item, seq, first, -}
+        const unsigned long long j = blk_first[h.x] + h.y;
+        if (j < used) {
+            const unsigned long long at = item_offs[h.x] + h.z;
+            desc[j] = make_uint4((uint32_t)b, min(BLK_EVENTS, ev_counts[h.x] - h.y * BLK_EVENTS), (uint32_t)at, (uint32_t)(at >> 32));
+        }
+    }
+}
+
+// k_expand's contract from block descriptors and two-entry lists.  Per warp, U blocks: descriptor, events, output_pos
+// of the slot and the list's pair entry are four dependent loads, issued for all U blocks before any is expanded; only
+// lists of three or more (class 3) walk the outputs from the head.  No shared memory: a CTA must fit beside a resident
+// scan CTA, whose staged records leave a few KiB of the carveout at most (staging a warp's run of tuples in 1 KiB for
+// 16-byte stores kept the placement of step s off the SMs of the scan of step s+1: the pipelined step got slower).
+constexpr uint32_t EXP_THREADS = 256;
+template <bool OVERLAP, int U>
+__global__ void __launch_bounds__(EXP_THREADS) k_expand_desc(const uint32_t* pool, const ScanCtrl* ctrl, uint32_t pool_blocks,
+                                                            const uint4* desc, const unsigned long long* item_offs,
+                                                            uint64_t n_items, unsigned long long out_cap, const unsigned long long* base,
+                                                            uint32_t* out_words, const unsigned long long* pad_like,
+                                                            const uint4* pairs, const uint4* outputs, const uint32_t* opos_tab) {
+    if (ctrl->overflow) return;
+    const unsigned long long b0m = base ? *base : 0ull;
+    if (b0m + item_offs[n_items] > out_cap) return;
+    out_words += b0m * 3ull;
+    if (pad_like) out_words += (*pad_like * 3ull) & 3ull;  // staged copy for k_push (k_gather)
+    const uint32_t used = min(ctrl->blk_cursor, pool_blocks);
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t warp = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const uint64_t n_warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t b0 = warp * U; b0 < used; b0 += n_warps * U) {
+        uint4 dsc[U], p[U];
+        uint2 ev[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            dsc[u] = desc[b0 + u < used ? b0 + u : b0];
+            if (b0 + u >= used) dsc[u].y = 0;
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+            ev[u] = lane < dsc[u].y ? reinterpret_cast<const uint2*>(pool + (uint64_t)dsc[u].x * BLK_WORDS + BLK_HDR_WORDS)[lane]
+                                    : make_uint2(0u, 0u);
+        uint32_t op[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) op[u] = lane < dsc[u].y ? ld_u32(opos_tab + (ev[u].y & QSLOT_MASK)) : 0u;
+#pragma unroll
+        for (int u = 0; u < U; ++u) p[u] = op[u] ? ld_u4(pairs + (op[u] - 1)) : make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            if (!dsc[u].y) continue;  // (warp-uniform)
+            const uint32_t cls = OVERLAP ? p[u].w >> PAIR_CLASS_SHIFT : (op[u] ? 1u : 0u);
+            uint4 r = make_uint4(0u, 0u, 0u, 0u);
+            if (cls == 3u) r = ld_u4(outputs + (op[u] - 1));  // head record: the chain word is the length
+            const uint32_t len = cls == 3u ? r.w : cls;
+            uint32_t inc = len;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t t = __shfl_up_sync(0xffffffffu, inc, d);
+                if (lane >= (uint32_t)d) inc += t;
+            }
+            uint32_t* w = out_words + (((unsigned long long)dsc[u].w << 32 | dsc[u].z) + (inc - len)) * 3ull;
+            const uint32_t end = ev[u].x;
+            if (cls == 1u || cls == 2u) {
+                w[0] = end - p[u].y;
+                w[1] = end;
+                w[2] = p[u].x;
+                if (cls == 2u) {
+                    w[3] = end - (p[u].w & PAIR_LEN_MASK);
+                    w[4] = end;
+                    w[5] = p[u].z;
+                }
+            } else if (cls == 3u) {
+                for (uint32_t k = 0;;) {
+                    w[0] = end - r.y;
+                    w[1] = end;
+                    w[2] = r.x;
+                    if (++k == len) break;
+                    w += 3;
+                    r = ld_u4(outputs + (r.z - 1));
+                }
+            }
+        }
+    }
+}
+
 // The exchange step proper: `total` dense 12-byte tuples from local memory to out_words + 3 * base in (peer)
 // memory, as DESTINATION-ALIGNED 16-byte stores -- a warp store is 512 contiguous bytes, whole 128-byte lines on
 // NVLink.  (k_gather's own stores are 4 bytes per lane at the 4-byte alignment of a tuple array: as peer stores
@@ -1071,6 +1166,7 @@ struct Workspace {
     DevBuf counts, ev_counts, tiles, ctrl, pool;  // ev_counts: events per item (event blocks)
     DevBuf nseg, seg_first, item_hay, item_beg, item_offs, n_items_dev;  // segment table, per-item offsets
     DevBuf blk_first, blkmap, tiles2;  // pool blocks in output order (k_blk_index)
+    DevBuf desc;                       // ... as block descriptors (k_blk_desc, event blocks)
     DevBuf stage;  // shard groups: the job's dense matches, pushed to the gathering rank by k_push
     DevBuf items_rk, total_rk;  // COUNT / FIRST: per-item results, the batch's total (u64)
     DevBuf slot_hist, rec_hist, hist_acc;  // HIST: per compact slot, per output record; host form: the batch's histogram
@@ -1084,6 +1180,7 @@ struct Workspace {
     uint64_t job_cap = 0;
     bool job_seg = false, job_ordered = false, job_open = false, job_placed = false;
     bool job_events = false;
+    bool job_desc = false;  // ordered event blocks with descriptors: k_expand_desc places them
     bool refused = false;  // finish_scan: a haystack passed 2^32 matches (*needed exact, status DACH_INVALID_ARGUMENT)
     int job_mode = 0;  // the pool holds event blocks (StdMachine3): k_expand places them, not k_gather
     cudaStream_t job_stream = nullptr;
@@ -1107,7 +1204,7 @@ struct Workspace {
     }
     void release() {
         for (DevBuf* b : {&counts, &ev_counts, &tiles, &ctrl, &pool, &text, &offs, &out, &out_offs, &nseg, &seg_first, &item_hay, &item_beg,
-                          &item_offs, &n_items_dev, &blk_first, &blkmap, &tiles2, &stage, &items_rk, &total_rk, &slot_hist, &rec_hist,
+                          &item_offs, &n_items_dev, &blk_first, &blkmap, &desc, &tiles2, &stage, &items_rk, &total_rk, &slot_hist, &rec_hist,
                           &hist_acc})
             if (b->p) {
                 cudaFree(b->p);
@@ -1155,6 +1252,7 @@ struct dach_dev {
     uint32_t* d_root = nullptr;
     uint4* d_crec = nullptr;
     uint32_t* d_opos = nullptr;
+    uint4* d_pairs = nullptr;  // two-entry output lists (nullptr: a pattern length reaches PAIR_CLASS_SHIFT)
     uint32_t* d_id_in = nullptr;   // crate slot -> compact slot (stream chunks)
     uint32_t* d_id_out = nullptr;  // compact slot -> crate slot
     uint32_t hot_slots = 0;        // size of the hot region of the compact image
@@ -1178,6 +1276,8 @@ struct dach_dev {
     // StdMachine3's matches path: 0 = events stored at their landing (k_scan_direct) when the scan runs one CTA per
     // SM, 1 = through the per-lane event queue (scan_machine with EventOps)
     int64_t opt_event_queue = 0;
+    int64_t opt_expand_desc = 1;  // ordered event blocks: 1 = k_expand_desc (descriptors, pairs), 0 = k_expand
+    int64_t opt_expand_u = 2;     // blocks in flight per warp of k_expand_desc (2, 4 or 8); 2: 60 registers, fits beside a scan CTA
     // HIST on the lane machines: events of the leading compact slots are counted in shared memory per CTA (4 B
     // each, next to the hot records and the queues) before they reach global memory.  0 = off.
     int64_t opt_hist_smem = 1024;
@@ -1596,6 +1696,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     W.job_seg = false;
     W.job_ordered = false;
     W.job_events = false;
+    W.job_desc = false;
     W.job_stream = st;
     W.job_open = true;
     if (!ensure(W.ctrl, sizeof(ScanCtrl)) || !ensure(W.item_offs, 16)) return DACH_CUDA_ERROR;
@@ -1716,8 +1817,11 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     d->launches += 4;
     // batches whose match blocks stay in L2 anyway are copied in pool order (four launches fewer)
     const bool ordered = d->opt_gather_ordered >= 2 || (d->opt_gather_ordered == 1 && text_bytes >= (256ull << 20));
+    // ordered event blocks are placed from descriptors (k_blk_desc) if the image has two-entry lists
+    const bool use_desc = ordered && events && d->d_pairs && d->opt_expand_desc != 0;
     if (ordered) {
-        if (!ensure(W.blk_first, (n_items_max + 1) * 8) || !ensure(W.blkmap, (size_t)pool_blocks * 4) || !ensure(W.tiles2, n_tiles * 8))
+        if (!ensure(W.blk_first, (n_items_max + 1) * 8) || !ensure(W.tiles2, n_tiles * 8) ||
+            !(use_desc ? ensure(W.desc, (size_t)pool_blocks * 16) : ensure(W.blkmap, (size_t)pool_blocks * 4)))
             return DACH_CUDA_ERROR;
         unsigned long long* tiles2 = static_cast<unsigned long long*>(W.tiles2.p);
         unsigned long long* blk_first = static_cast<unsigned long long*>(W.blk_first.p);
@@ -1730,7 +1834,11 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
             k_offsets_scan_tiles<<<1, kScanThreads, 0, st>>>(tiles2, n_tiles);
             k_offsets_apply<BLK_MATCHES><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(P.counts, n_items_max, tiles2, blk_first);
         }
-        k_blk_index<<<d->sm_count * 8, 256, 0, st>>>(P.pool, P.ctrl, pool_blocks, blk_first, static_cast<uint32_t*>(W.blkmap.p));
+        if (use_desc)
+            k_blk_desc<<<d->sm_count * 8, 256, 0, st>>>(P.pool, P.ctrl, pool_blocks, blk_first, P.ev_counts, item_offs,
+                                                        static_cast<uint4*>(W.desc.p));
+        else
+            k_blk_index<<<d->sm_count * 8, 256, 0, st>>>(P.pool, P.ctrl, pool_blocks, blk_first, static_cast<uint32_t*>(W.blkmap.p));
         d->launches += 4;
     }
     if (!cuda_ok(cudaGetLastError(), "kernel launch")) return DACH_CUDA_ERROR;
@@ -1739,6 +1847,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     W.job_seg = seg;
     W.job_ordered = ordered;
     W.job_events = events;
+    W.job_desc = use_desc;
     W.job_mode = mode;
     W.job_pool_blocks = pool_blocks;
     return DACH_OK;
@@ -1774,7 +1883,15 @@ int enqueue_place(dach_dev* d, Workspace& W, dach_match* d_out, uint64_t out_cap
             g_cap = W.job_cap;
         }
         const unsigned long long* pad_like = staged ? d_base : nullptr;
-        if (W.job_events) {
+        if (W.job_desc) {
+            const uint4* desc = static_cast<const uint4*>(W.desc.p);
+            const int u = d->opt_expand_u >= 8 ? 8 : d->opt_expand_u <= 2 ? 2 : 4;
+            const bool ov = W.job_mode == M_OVERLAPPING;
+            auto kern = ov ? (u == 8 ? k_expand_desc<true, 8> : u == 2 ? k_expand_desc<true, 2> : k_expand_desc<true, 4>)
+                           : (u == 8 ? k_expand_desc<false, 8> : u == 2 ? k_expand_desc<false, 2> : k_expand_desc<false, 4>);
+            kern<<<gather_grid, EXP_THREADS, 0, st>>>(pool, ctrl, W.job_pool_blocks, desc, item_offs, n_items, g_cap, g_base, out_words,
+                                                      pad_like, d->d_pairs, d->d_outputs, d->d_opos);
+        } else if (W.job_events) {
             const uint32_t* ev_counts = static_cast<const uint32_t*>(W.ev_counts.p);
             if (W.job_mode == M_OVERLAPPING)
                 k_expand<true, 2><<<gather_grid, 256, 0, st>>>(pool, ctrl, W.job_pool_blocks, ev_counts, item_offs, n_items, g_cap, g_base,
@@ -2621,9 +2738,9 @@ int dach_dev_upload(const dach_pma* pma, int device, dach_dev** out) {
         d->sm_count = prop.multiProcessorCount;
         d->smem_optin = prop.sharedMemPerBlockOptin;
         // one allocation for the whole image, 512-byte aligned parts
-        constexpr int kParts = 8;
+        constexpr int kParts = 9;
         const std::vector<uint32_t>* parts[kParts] = {&img.rec, &img.outputs, &img.root_table, &img.mapper, &img.crec, &img.opos_tab,
-                                                       &img.new_of_old, &img.old_of_new};
+                                                       &img.new_of_old, &img.old_of_new, &img.pairs};
         size_t part_off[kParts], total = 0;
         for (int i = 0; i < kParts; ++i) {
             part_off[i] = total;
@@ -2641,6 +2758,7 @@ int dach_dev_upload(const dach_pma* pma, int device, dach_dev** out) {
             char* b = static_cast<char*>(d->image_base);
             d->d_rec = reinterpret_cast<uint4*>(b + part_off[0]);
             d->d_outputs = reinterpret_cast<uint4*>(b + part_off[1]);
+            if (!img.pairs.empty()) d->d_pairs = reinterpret_cast<uint4*>(b + part_off[8]);
             d->d_root = reinterpret_cast<uint32_t*>(b + part_off[2]);
             d->d_mapper = reinterpret_cast<uint32_t*>(b + part_off[3]);
             if (!img.crec.empty()) {
@@ -3269,6 +3387,10 @@ int dach_dev_set_option(dach_dev* d, const char* name, int64_t value) {
         d->opt_hot_entries = value;
     else if (k == "event_queue")
         d->opt_event_queue = value;
+    else if (k == "expand_desc")
+        d->opt_expand_desc = value;
+    else if (k == "expand_u")
+        d->opt_expand_u = value;
     else if (k == "hist_smem")
         d->opt_hist_smem = value;
     else if (k == "df_pairs")

@@ -104,7 +104,8 @@ def event_blocks():
     for mode in (D.FIND, D.FIND_OVERLAPPING, D.FIND_OVERLAPPING_NO_SUFFIX):
         ref = opma.scan_batch(ORC[mode], text, offs, want_matches=True)
         for opts in ({"gather_ordered": 0}, {"gather_ordered": 2}, {"gather_ordered": 2, "seg_len": 64}, {"event_queue": 1},
-                     {"event_queue": 1, "seg_len": 64}):
+                     {"event_queue": 1, "seg_len": 64}, {"gather_ordered": 2, "expand_desc": 0},
+                     {"gather_ordered": 2, "expand_u": 8}):
             for k, v in opts.items():
                 pma.set_option(k, v)
             r = pma.scan_batch_host(mode, text, offs)
@@ -112,6 +113,8 @@ def event_blocks():
             n_scans += 1
             pma.set_option("seg_len", 0)
             pma.set_option("event_queue", 0)
+            pma.set_option("expand_desc", 1)
+            pma.set_option("expand_u", 2)
         pma.set_option("gather_ordered", 1)
 
 
