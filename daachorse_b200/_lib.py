@@ -21,7 +21,7 @@ SYMBOLS = [
     "dach_dev_upload", "dach_dev_free", "dach_dev_image_bytes", "dach_dev_scan_batch", "dach_dev_scan_stream",
     "dach_dev_count_stream", "dach_dev_first_stream", "dach_dev_hist_stream", "dach_scan_batch_host", "dach_dev_count_batch", "dach_count_batch_host", "dach_dev_first_batch", "dach_first_batch_host",
     "dach_dev_hist_batch", "dach_hist_batch_host", "dach_dev_df_batch", "dach_df_batch_host", "dach_dev_last_df_windows",
-    "dach_dev_kernel_launches", "dach_dev_last_scan_kernel_ms",
+    "dach_dev_mask_batch", "dach_mask_batch_host", "dach_dev_kernel_launches", "dach_dev_last_scan_kernel_ms",
     "dach_dev_last_total_ms", "dach_dev_last_h2d_bytes", "dach_dev_last_d2h_bytes",
     "dach_dev_set_option", "dach_last_error", "dach_abi_version",
     "dach_job_create", "dach_job_free", "dach_job_scan", "dach_job_place", "dach_job_wait", "dach_job_scan_kernel_ms", "dach_job_push_ms", "dach_job_times",
@@ -95,8 +95,11 @@ def load():
     L.dach_dev_df_batch.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_uint64, C.c_uint64, vp, C.c_uint64, C.POINTER(C.c_uint64), vp]
     L.dach_df_batch_host.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_uint64, vp, C.c_uint64, C.POINTER(C.c_uint64)]
     L.dach_dev_last_df_windows.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    L.dach_dev_mask_batch.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, C.c_uint64, C.c_uint8, vp, vp]
+    L.dach_mask_batch_host.argtypes = [vp, C.c_int, vp, vp, C.c_uint64, C.c_uint8, vp]
     for name in ("dach_dev_count_batch", "dach_count_batch_host", "dach_dev_first_batch", "dach_first_batch_host",
-                 "dach_dev_hist_batch", "dach_hist_batch_host", "dach_dev_df_batch", "dach_df_batch_host", "dach_dev_last_df_windows"):
+                 "dach_dev_hist_batch", "dach_hist_batch_host", "dach_dev_df_batch", "dach_df_batch_host", "dach_dev_last_df_windows",
+                 "dach_dev_mask_batch", "dach_mask_batch_host"):
         getattr(L, name).restype = C.c_int
     L.dach_dev_kernel_launches.argtypes = [vp]
     L.dach_dev_kernel_launches.restype = C.c_uint64

@@ -594,6 +594,63 @@ class _Automaton:
         _check(_lib.load().dach_dev_last_df_windows(self.device_handle(device), C.byref(w), C.byref(r)))
         return w.value, r.value
 
+    # -- masked text (no match list) ----------------------------------------------------------------
+    def _fill_byte(self, fill):
+        if isinstance(fill, (bytes, str)) and len(fill) == 1:
+            fill = ord(fill)
+        if isinstance(fill, bool) or not isinstance(fill, (int, np.integer)) or not 0 <= int(fill) <= 255:
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "fill must be one byte (an int in 0..255)")
+        if self._charwise and fill >= 0x80:
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "the fill of a charwise automaton must be ASCII (below 0x80)")
+        return int(fill)
+
+    def mask_batch_host(self, mode, text, offs, fill=ord("*"), out=None, device=None):
+        """``text`` with every byte a match of iterator ``mode`` covers set to ``fill``, host buffers in and out:
+        ``np.uint8`` of ``text``'s size (``out``: optional preallocated one).  Bytes outside the haystacks are copied."""
+        fill = self._fill_byte(fill)
+        text, offs, n = self._host_batch_args(mode, text, offs)
+        if int(offs[-1]) > text.size:  # the copy reads text[0, offs[n]) even when n == 0
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "offsets must stay inside the text")
+        if out is None:
+            out = np.empty(text.size, dtype=np.uint8)
+        elif out.dtype != np.uint8 or out.ndim != 1 or out.size < text.size or not out.flags.c_contiguous or not out.flags.writeable:
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "out must be a writable contiguous 1-d uint8 array of at least text.size bytes")
+        if out.size and text.size and np.shares_memory(out, text):
+            raise DaachorseError(_lib.INVALID_ARGUMENT, "out must not overlap text (masking in place is not supported)")
+        L = _lib.load()
+        d = self.device_handle(device)
+        _check(L.dach_mask_batch_host(d, mode, _ptr(text), C.c_void_p(offs.ctypes.data), n, fill, _ptr(out)))
+        end = int(offs[-1])
+        out[end:text.size] = text[end:]
+        return out
+
+    def mask_batch_device(self, mode, text, offs, fill=ord("*"), out=None, stream=None):
+        """Device-resident form of ``mask_batch_host``: ``text`` / ``offs`` as in ``scan_batch_device``; returns a uint8
+        CUDA tensor of ``text``'s size (``out``: optional preallocated one, which must not overlap ``text``)."""
+        import torch
+
+        fill = self._fill_byte(fill)
+        self._assert_mode(mode)
+        dev = text.device.index if text.device.index is not None else torch.cuda.current_device()
+        if out is None:
+            out = torch.empty(text.numel(), dtype=torch.uint8, device=text.device)
+        _check_device_batch(text, offs, dev, masked=out)
+        d = self.device_handle(dev)
+        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
+        _check(_lib.load().dach_dev_mask_batch(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), offs.numel() - 1,
+                                               text.numel(), fill, C.c_void_p(out.data_ptr()), st))
+        return out
+
+    def mask_batch(self, haystacks, fill=b"*", mode=None):
+        """Every haystack with the bytes its matches cover replaced by ``fill``: a list of ``bytes``, or of ``str`` for
+        a charwise automaton (whose fill must be ASCII); ``mode=None`` as in ``count_batch``."""
+        haystacks = list(haystacks)
+        fill = self._fill_byte(fill)
+        blob, offs = _pack(haystacks, self._charwise)
+        masked = self.mask_batch_host(self._default_mode(mode), blob, offs, fill=fill).tobytes()
+        res = [masked[int(offs[i]):int(offs[i + 1])] for i in range(len(haystacks))]
+        return [r.decode("utf-8") for r in res] if self._charwise else res
+
     def value_doc_counts_batch(self, haystacks, mode=None):
         """Haystacks containing each value: ``np.uint64[max value + 1]`` (for ``new`` automata: per pattern);
         ``mode=None`` as in ``count_batch``."""
@@ -742,7 +799,7 @@ def torch_int64():
 
 
 def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=None, pos=None, counts=None, first=None,
-                        found=None, hist=None, hist_len=0):
+                        found=None, hist=None, hist_len=0, masked=None):
     """Raw pointers cross the C ABI: a wrong dtype, stride or device would be silent garbage or a device fault."""
     import torch
 
@@ -756,7 +813,8 @@ def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=No
                             ("out", out, (torch.int32, torch.uint32)), ("out_offs", out_offs, (torch.int64, torch.uint64)),
                             ("state", state, (torch.int32, torch.uint32)), ("pos", pos, (torch.int32, torch.uint32)),
                             ("counts", counts, (torch.int64, torch.uint64)), ("first", first, (torch.int32, torch.uint32)),
-                            ("found", found, (torch.bool, torch.uint8)), ("hist", hist, (torch.int64,))):
+                            ("found", found, (torch.bool, torch.uint8)), ("hist", hist, (torch.int64,)),
+                            ("masked", masked, (torch.uint8,))):
         if t is None:
             continue
         if not t.is_cuda or t.device.index != dev_index:
@@ -776,6 +834,12 @@ def _check_device_batch(text, offs, dev_index, out=None, out_offs=None, state=No
         bad("first must have shape (n, 3)")
     if hist is not None and (hist.dim() != 1 or hist.numel() < hist_len):
         bad("hist must be 1-d with at least %d entries" % hist_len)
+    if masked is not None:
+        if masked.numel() < text.numel():
+            bad("the masked output must hold at least text.numel() bytes")
+        a, b = text.data_ptr(), masked.data_ptr()
+        if text.numel() and a < b + text.numel() and b < a + text.numel():
+            bad("the masked output must not overlap text (masking in place is not supported)")
 
 
 def _current_device():

@@ -82,7 +82,9 @@ using SinkOf = typename std::conditional<
     RK == RK_COUNT, CountSink,
     typename std::conditional<
         RK == RK_FIRST || RK == RK_FIRST_STREAM, FirstSink,
-        typename std::conditional<RK == RK_HIST, HistSink, typename std::conditional<RK == RK_DF, DfSink, Emitter>::type>::type>::type>::type;
+        typename std::conditional<
+            RK == RK_HIST, HistSink,
+            typename std::conditional<RK == RK_DF, DfSink, typename std::conditional<RK == RK_MASK, MaskSink, Emitter>::type>::type>::type>::type>::type;
 
 template <bool CHARWISE, int MODE, class SINK>
 __device__ __forceinline__ void scan_items(const ScanParams& P) {
@@ -103,6 +105,7 @@ __device__ __forceinline__ void scan_items(const ScanParams& P) {
         const uint32_t len = (uint32_t)(o1 - o0);
         T.open(P.text + o0);
         E.begin((uint32_t)item);
+        if constexpr (SINK::KIND == RK_MASK) E.base = P.mask_out + o0;
         if (MODE == M_LEFTMOST)
             scan_leftmost<CHARWISE>(P, V, T, E, len);
         else
@@ -1005,6 +1008,40 @@ __global__ void __launch_bounds__(256) k_count_hay(const unsigned long long* seg
         counts[h] = v;
     }
     add_block_total(v, total);
+}
+
+// ---- MASK: the text copied into the masked buffer before the scan fills its spans --------------------------------
+// dst[i] = src[i] for i < bytes, at any alignment of src and dst to each other.  A thread writes one 16-byte-aligned chunk
+// of dst with one 16-byte store, built from the two aligned 16-byte loads of src that cover it: the shift between them,
+// (src - dst) mod 16, is the same for every chunk.  A chunk whose loads or store would reach outside the buffers (at
+// most two at each end) goes byte by byte.  A refused call (bad offsets) writes nothing.
+__device__ __forceinline__ uint32_t word_of(const uint4& x, const uint4& y, uint32_t i) {  // word i of the 32 bytes x, y
+    const uint32_t lo = (i & 2u) ? ((i & 1u) ? x.w : x.z) : ((i & 1u) ? x.y : x.x);
+    const uint32_t hi = (i & 2u) ? ((i & 1u) ? y.w : y.z) : ((i & 1u) ? y.y : y.x);
+    return (i & 4u) ? hi : lo;
+}
+__global__ void __launch_bounds__(256) k_mask_copy(const uint8_t* src, uint8_t* dst, uint64_t bytes, const ScanCtrl* ctrl) {
+    if (ctrl->bad_offsets) return;
+    const uintptr_t s_lo = (uintptr_t)src, s_hi = s_lo + bytes, d_lo = (uintptr_t)dst, d_hi = d_lo + bytes;
+    const uintptr_t d0 = d_lo & ~(uintptr_t)15, delta = s_lo - d_lo;  // source byte of dst byte q: q + delta (mod 2^64)
+    const uint32_t sh = (uint32_t)delta & 15u, q = sh >> 2, r = (sh & 3u) * 8u;
+    const uint64_t n_chunks = (d_hi - d0 + 15) >> 4;
+    for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < n_chunks; c += (uint64_t)gridDim.x * blockDim.x) {
+        const uintptr_t d = d0 + (c << 4), a = (d + delta) & ~(uintptr_t)15;
+        if (d >= d_lo && d + 16 <= d_hi && a >= s_lo && a + (sh ? 32u : 16u) <= s_hi) {
+            const uint4 x = __ldg(reinterpret_cast<const uint4*>(a));
+            const uint4 y = sh ? __ldg(reinterpret_cast<const uint4*>(a + 16)) : x;
+            uint4 o;
+            o.x = __funnelshift_r(word_of(x, y, q), word_of(x, y, q + 1), r);
+            o.y = __funnelshift_r(word_of(x, y, q + 1), word_of(x, y, q + 2), r);
+            o.z = __funnelshift_r(word_of(x, y, q + 2), word_of(x, y, q + 3), r);
+            o.w = __funnelshift_r(word_of(x, y, q + 3), word_of(x, y, q + 4), r);
+            *reinterpret_cast<uint4*>(d) = o;
+        } else {
+            for (uintptr_t b = d; b < d + 16; ++b)
+                if (b >= d_lo && b < d_hi) *reinterpret_cast<uint8_t*>(b) = *reinterpret_cast<const uint8_t*>(b + delta);
+        }
+    }
 }
 
 __global__ void __launch_bounds__(256) k_first_hay(const unsigned long long* seg_first, const uint4* item_first, uint64_t n,
@@ -2221,9 +2258,12 @@ DfSet df_set(dach_dev* d, int i) {
 // d_state_io (stream chunks, dach_dev_*_stream): haystack i is the next chunk of stream i, resumed in and leaving its
 // state there as in enqueue_scan; FIRST then runs the caller's iterator to each chunk's last byte (RK_FIRST_STREAM)
 // and adds d_pos (or nothing) to its positions.  Stream chunks are never cut into segments.
+// rk = RK_MASK: d_masked (in the text's coordinates, like d_text) receives [text_lo, text_end) of the text, then `fill`
+// over every match; no post-pass.
 int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
                uint64_t text_bytes, const uint64_t* d_offs, uint64_t n, uint64_t* d_counts, dach_match* d_first, uint8_t* d_found,
-               cudaStream_t st, int key = 0, uint64_t* d_hist = nullptr, uint32_t* d_state_io = nullptr, const uint32_t* d_pos = nullptr) {
+               cudaStream_t st, int key = 0, uint64_t* d_hist = nullptr, uint32_t* d_state_io = nullptr, const uint32_t* d_pos = nullptr,
+               uint8_t* d_masked = nullptr, uint8_t fill = 0) {
     if (n > 0xfffffff0ull) {
         set_error("too many haystacks in one batch (max 2^32-16)");
         return DACH_INVALID_ARGUMENT;
@@ -2236,6 +2276,14 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
     cudaEventRecord(W.ev[0], st);
     cudaEventRecord(W.ev[3], st);
     unsigned long long* total = static_cast<unsigned long long*>(W.total_rk.p);
+    // MASK: the copy runs after the offsets check (it writes nothing if that fails) and before the scan
+    auto mask_copy = [&]() {
+        const uint64_t bytes = (uint64_t)(text_end - text_lo);
+        if (rk != RK_MASK || bytes == 0) return;
+        const uint64_t blocks = std::min<uint64_t>((bytes / 16 + 256) / 256, 16ull * d->sm_count);
+        k_mask_copy<<<(unsigned)blocks, 256, 0, st>>>(text_lo, d_masked + (text_lo - d_text), bytes, static_cast<const ScanCtrl*>(W.ctrl.p));
+        ++d->launches;
+    };
     if (n > 0) {
         int threads = (int)std::min<int64_t>(std::max<int64_t>(d->opt_threads, 32), kMaxThreads);
         threads = (threads / 32) * 32;
@@ -2299,9 +2347,12 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             P.df_slots = df_set(d, 0);
             P.df_keys = df_set(d, 1);
         }
+        P.mask_out = d_masked;
+        P.mask_fill = fill;
         const size_t smem = plan_smem(d, P, machine, std3, threads, ctas_per_sm, 1, hist_k);
         k_check_offsets<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_offs, n, (uint64_t)(text_end - d_text), P.ctrl);
         ++d->launches;
+        mask_copy();
         if (seg) enqueue_seg_table(d, W, d_offs, n, seg_len, 0, P, st);
         cudaEventRecord(W.ev[3], st);
         const int which = std3 ? 3 : machine ? 1 : 0;
@@ -2309,6 +2360,7 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         if (!cuda_ok(rk == RK_COUNT  ? launch_rk<RK_COUNT>(which, d->charwise, mmode, P, grid, t, smem, st)
                      : rk == RK_HIST ? launch_rk<RK_HIST>(which, d->charwise, mmode, P, grid, t, smem, st)
                      : rk == RK_DF   ? launch_rk<RK_DF>(which, d->charwise, mmode, P, grid, t, smem, st)
+                     : rk == RK_MASK ? launch_rk<RK_MASK>(which, d->charwise, mmode, P, grid, t, smem, st)
                      : d_state_io    ? launch_first_stream(d->charwise, mmode, P, grid, t, smem, st)
                                      : launch_rk<RK_FIRST>(which, d->charwise, mmode, P, grid, t, smem, st),
                      "k_scan launch"))
@@ -2343,7 +2395,8 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             if (!cuda_ok(cudaMemsetAsync(d->df_n.p, 0, 8, st), "memset pair counts")) return DACH_CUDA_ERROR;
         } else if (rk == RK_COUNT)
             k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(d_counts), total, P.ctrl);
-        else if (d_state_io)
+        else if (rk == RK_MASK) {
+        } else if (d_state_io)
             k_first_stream<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(P.item_first, n, d_pos, reinterpret_cast<uint32_t*>(d_first), d_found, total, P.ctrl);
         else
             k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(d_first), d_found, total, P.ctrl);
@@ -2351,6 +2404,10 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         else ++d->launches;                                    // the scan
         if (!cuda_ok(cudaGetLastError(), "kernel launch")) return DACH_CUDA_ERROR;
     } else {
+        if (rk == RK_MASK) {  // no haystack: every byte is outside one
+            mask_copy();
+            if (!cuda_ok(cudaGetLastError(), "kernel launch")) return DACH_CUDA_ERROR;
+        }
         cudaEventRecord(W.ev[1], st);
     }
     cudaEventRecord(W.ev[2], st);
@@ -2437,6 +2494,78 @@ int rk_batch_host_impl(dach_dev* d, int rk, int mode, const uint8_t* text, const
     for (Workspace& w : d->slot)
         if (!cuda_ok(cudaStreamSynchronize(w.stream), "D2H")) return DACH_CUDA_ERROR;
     if (total) *total = sum;
+    return DACH_OK;
+}
+
+// MASK: the fill byte of a charwise automaton keeps UTF-8 valid, and the masked buffer does not overlap the text (a lane
+// that has not read its bytes yet would see another lane's fill: spans reach back into the segment before theirs)
+int check_mask(const dach_dev* d, const uint8_t* text, uint64_t text_bytes, uint8_t fill, const uint8_t* out) {
+    if (d->charwise && fill >= 0x80) {
+        set_error("the fill byte of a charwise automaton must be below 0x80 (the masked text stays valid UTF-8)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    if (text_bytes && (uintptr_t)out < (uintptr_t)text + text_bytes && (uintptr_t)text < (uintptr_t)out + text_bytes) {
+        set_error("the masked buffer overlaps the text (masking in place is not supported)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    return DACH_OK;
+}
+
+// MASK of a host-buffer batch: the slices of dach_scan_batch_host; each slice's masked bytes come back into out
+int mask_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, uint8_t fill, uint8_t* out) {
+    if (!d || !offs || (offs[n] && (!text || !out))) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    int rc = check_mask(d, text, offs[n], fill, out);
+    if (rc) return rc;
+    rc = check_mode(d, mode);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(d->mu);
+    DeviceGuard g(d->device);
+    if (!g.ok) return DACH_CUDA_ERROR;
+    d->last_h2d = d->last_d2h = 0;
+    if (n == 0) {
+        if (offs[0]) memcpy(out, text, offs[0]);
+        return DACH_OK;
+    }
+    rc = check_host_offsets(offs, n);
+    if (rc) return rc;
+    struct Drain {  // no exit may leave copies of the caller's buffers in flight
+        dach_dev* d;
+        ~Drain() {
+            for (Workspace& w : d->slot)
+                if (w.stream) cudaStreamSynchronize(w.stream);
+        }
+    } drain_on_exit{d};
+    const std::vector<Slice> slices = cut_slices(d, mode, offs, n);
+    for (Workspace& w : d->slot)
+        if (!w.init(true)) return DACH_CUDA_ERROR;
+    if (offs[0]) memcpy(out, text, offs[0]);  // bytes before the first haystack
+    double t_reuse = 0;
+    auto issue_h2d = [&](size_t k) -> bool {
+        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
+    };
+    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
+    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
+    for (size_t k = 0; k < slices.size(); ++k) {
+        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
+        Workspace& W = d->slot[k % dach_dev::kSlots];
+        const Slice& s = slices[k];
+        const uint64_t tb = offs[s.last] - offs[s.first], ns = s.last - s.first;
+        if (!ensure(W.out, tb + 16)) return DACH_CUDA_ERROR;
+        const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
+        rc = enqueue_rk(d, W, RK_MASK, mode, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb, tb,
+                        static_cast<const uint64_t*>(W.offs.p), ns, nullptr, nullptr, nullptr, W.stream, 0, nullptr, nullptr, nullptr,
+                        static_cast<uint8_t*>(W.out.p) - offs[s.first], fill);
+        if (!rc) rc = finish_rk(d, W, nullptr);
+        if (rc) return rc;
+        if (tb && !cuda_ok(cudaMemcpyAsync(out + offs[s.first], W.out.p, tb, cudaMemcpyDeviceToHost, W.stream), "D2H masked text"))
+            return DACH_CUDA_ERROR;
+        d->last_d2h += tb;
+    }
+    for (Workspace& w : d->slot)
+        if (!cuda_ok(cudaStreamSynchronize(w.stream), "D2H")) return DACH_CUDA_ERROR;
     return DACH_OK;
 }
 
@@ -2991,6 +3120,30 @@ int dach_dev_last_df_windows(const dach_dev* d, uint64_t* windows, uint64_t* res
     if (windows) *windows = d->last_df_windows;
     if (rescans) *rescans = d->last_df_rescans;
     return DACH_OK;
+}
+
+int dach_dev_mask_batch(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                        uint8_t fill, uint8_t* d_out, void* stream) {
+    if (!d || !d_offs || (text_bytes && (!d_text || !d_out))) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    int rc = check_mask(d, d_text, text_bytes, fill, d_out);
+    if (rc) return rc;
+    rc = check_mode(d, mode);
+    if (rc) return rc;
+    return guarded([&]() -> int {
+        std::lock_guard<std::mutex> lk(d->mu);
+        DeviceGuard g(d->device);
+        if (!g.ok) return DACH_CUDA_ERROR;
+        const int r = enqueue_rk(d, d->ws, RK_MASK, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, nullptr, nullptr,
+                                 nullptr, static_cast<cudaStream_t>(stream), 0, nullptr, nullptr, nullptr, d_out, fill);
+        return r ? r : finish_rk(d, d->ws, nullptr);
+    });
+}
+
+int dach_mask_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, uint8_t fill, uint8_t* out) {
+    return guarded([&]() -> int { return mask_batch_host_impl(d, mode, text, offs, n, fill, out); });
 }
 
 // ---- asynchronous jobs ------------------------------------------------------------------------------

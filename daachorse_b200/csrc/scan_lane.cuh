@@ -16,8 +16,8 @@
 //   - StdMachine3  the default (kernel=3): no probe-state flags, one stop bit, cursor = address word, records from
 //                  the hot-first image (optionally its front from shared memory); probe / resolve are separate so
 //                  that k_scan_duo can keep two fetches in flight; serves stream chunks
-//   - SinkOps      COUNT / FIRST / HIST / DF on StdMachine3, LmMachine, CwMachine: their drain() / begin_item()
-//                  for the other result kinds (sinks: Emitter, CountSink, FirstSink, HistSink, DfSink)
+//   - SinkOps      COUNT / FIRST / HIST / DF / MASK on StdMachine3, LmMachine, CwMachine: their drain() / begin_item()
+//                  for the other result kinds (sinks: Emitter, CountSink, FirstSink, HistSink, DfSink, MaskSink)
 //   - EventOps     the matches path of StdMachine3: events stored into event blocks (EventSink), expanded after
 //                  the scan by k_expand
 //
@@ -176,6 +176,10 @@ struct ScanParams {
     // pairs (lane per haystack, and k_df_expand from the slot pairs); df_key_value: the key is the value
     uint32_t df_key_value;
     DfSet df_slots, df_keys;
+    // MASK (MaskSink): the masked copy of the text, in the text's coordinates (mask_out + offs[h] is haystack h's
+    // first byte), and the fill byte
+    uint8_t* mask_out;
+    uint32_t mask_fill;
 };
 
 // What a scan produces (compile time): every match (Emitter), the number of matches (CountSink), the first
@@ -186,6 +190,8 @@ constexpr int RK_MATCHES = 0, RK_COUNT = 1, RK_FIRST = 2, RK_HIST = 3, RK_DF = 4
 // FIRST on stream chunks (dach_dev_first_stream): a FirstSink, but the item is scanned to its last byte, because the
 // next chunk resumes in the state after it
 constexpr int RK_FIRST_STREAM = 5;
+// MASK (dach_dev_mask_batch): every byte a match covers is overwritten with a fill byte in a copy of the text (MaskSink)
+constexpr int RK_MASK = 6;
 
 // L2 eviction policies (64-bit descriptors made once per device by k_make_policies, dev_scan.cu):
 //   [0] automaton image (records, output_pos, outputs, mapper): evict_last -- the scan is latency-bound on
@@ -594,6 +600,37 @@ DACH_HD void emit_chain(const ScanParams& P, DfSink& E, uint32_t opos, uint32_t)
     }
 }
 
+// MASK: the bytes a reported match covers become P.mask_fill in P.mask_out, whose copy of the text k_mask_copy
+// (dev_scan.cu) has written before the scan.  An event -- and, on the lane-per-haystack loops, an output list -- fills
+// the span of its list head, [end - length, end): for find_overlapping every other entry of the list is a suffix of
+// the head, so the head's span is the union of the list's spans; the other iterators report the head alone.
+//   lane machines: event(end, slot) loads output_pos of the slot and the head's length (two dependent loads);
+//   lane per haystack: emit_head / emit_chain fill the head's span.
+// Lanes that fill the same byte store the same value, so the stores need no atomics; none ever reads back a byte.
+// The start is clamped at the haystack's first byte: a deserialized automaton may carry a length above `end`.
+struct MaskSink {
+    static constexpr int KIND = RK_MASK;
+    uint8_t* base = nullptr;  // the masked copy of the item's haystack (set by the kernel's item start)
+    uint32_t item = 0;
+    DACH_HD void begin(uint32_t item_id) { item = item_id; }
+    DACH_HD void finish(const ScanParams&) {}
+    DACH_HD bool stopped() const { return false; }
+    // only zero-length matches (ROOT's empty pattern) arrive here: they cover no byte
+    DACH_HD void emit(const ScanParams&, uint32_t, uint32_t, uint32_t) {}
+    DACH_HD void span(const ScanParams& P, uint32_t end, uint32_t len) {
+        const uint8_t f = (uint8_t)P.mask_fill;
+        for (uint32_t i = len < end ? end - len : 0u; i < end; ++i) base[i] = f;
+    }
+    DACH_HD void event(const ScanParams& P, uint32_t end, uint32_t slot) {
+        const uint32_t opos = ld_u32(P.opos_tab + slot);
+        span(P, end, ld_u32(reinterpret_cast<const uint32_t*>(P.outputs + (opos - 1)) + 1));
+    }
+};
+DACH_HD void emit_head(const ScanParams& P, MaskSink& E, uint32_t opos, uint32_t end) { E.span(P, end, ld_u4(P.outputs + (opos - 1)).y); }
+DACH_HD void emit_chain(const ScanParams& P, MaskSink& E, uint32_t opos, uint32_t end) {
+    if (opos != 0) emit_head(P, E, opos, end);
+}
+
 // ---- record access: leading `hot_n` records come from shared memory --------------------
 struct RecView {
     const uint4* glob;
@@ -729,6 +766,9 @@ DACH_HD void scan_standard(const ScanParams& P, const RecView& V, TextWin& T, SI
             emit_head(P, E, root_opos, 0);
             return;
         }
+    }
+    if constexpr (SINK::KIND == RK_MASK) {
+        if (MODE == M_FIND && root_opos) return;  // only zero-length matches: nothing to mask
     }
     if constexpr (SINK::KIND == RK_HIST) {
         if (MODE == M_FIND && root_opos) {  // one match of ROOT's record per boundary
@@ -2360,6 +2400,8 @@ struct StdMachine3 {
 //          here; dev_scan.cu's post-passes turn slot counts into output-record counts.
 //   DF     puts (haystack, slot) of every reportable event into the window's pair set (DfSink::event),
 //          the haystack of a segment being item_hay[item]; k_df_expand maps slots to keys after the scan.
+//   MASK   fills the head's span of every reportable event in the masked copy (MaskSink::event); begin_item() points
+//          the sink at the item's haystack, so a segment's spans may reach back into the segment before it.
 //   FIRST_STREAM  (stream chunks) keeps the full queue and drains like COUNT: the head of the item's first
 //          event is its answer, and the lane goes on to the chunk's last byte, whose state the next chunk
 //          resumes in.  A chunk is never cut into segments and starts with an empty queue (the incoming
@@ -2373,7 +2415,8 @@ struct SinkOps {
     using Sink = typename std::conditional<
         RK == RK_COUNT, CountSink,
         typename std::conditional<RK == RK_FIRST || RK == RK_FIRST_STREAM, FirstSink,
-                                  typename std::conditional<RK == RK_HIST, HistSink, DfSink>::type>::type>::type;
+                                  typename std::conditional<RK == RK_HIST, HistSink,
+                                                            typename std::conditional<RK == RK_DF, DfSink, MaskSink>::type>::type>::type>::type;
 
     template <class LANE>
     static DACH_HD void begin_item(LANE& L, const ScanParams& P, const StdEnv& Ev, Sink& E, uint64_t item, const uint8_t* emu_lo) {
@@ -2383,6 +2426,7 @@ struct SinkOps {
         if constexpr (RK == RK_DF) {
             if (P.item_hay) E.hay = P.item_hay[item];  // a segment counts for its haystack
         }
+        if constexpr (RK == RK_MASK) E.base = P.mask_out + P.offs[P.item_hay ? P.item_hay[item] : item];
         if constexpr (RK == RK_FIRST) {
             if (L.qn) {  // ROOT's list at position 0 (an empty pattern): reportable at once
                 E.emit(P, 0, 0, ld_u4(P.outputs + (ld_u32(Ev.opos + (Ev.q[0].opos & QSLOT_MASK)) - 1)).x);
@@ -2412,6 +2456,14 @@ struct SinkOps {
                 if (j < L.qn) {
                     const QEntry e = Ev.q[j * Ev.q_stride];
                     if (e.end >= L.from) E.event(P, e.opos & QSLOT_MASK);  // the entry holds the slot
+                }
+            }
+            L.qn = 0;
+        } else if constexpr (RK == RK_MASK) {
+            for (uint32_t j = 0; j < (uint32_t)LANE_Q; ++j) {
+                if (j < L.qn) {
+                    const QEntry e = Ev.q[j * Ev.q_stride];
+                    if (e.end >= L.from) E.event(P, e.end, e.opos & QSLOT_MASK);
                 }
             }
             L.qn = 0;

@@ -305,6 +305,27 @@ int dach_df_batch_host(dach_dev *dev, int mode, int key, const uint8_t *text, co
                        uint64_t n, uint64_t *df, uint64_t n_df, uint64_t *total);
 int dach_dev_last_df_windows(const dach_dev *dev, uint64_t *windows, uint64_t *rescans);
 
+/* ---- masked text ------------------------------------------------------------------------------
+ *
+ * Every byte covered by a match replaced by a fill byte, with no match list (redaction, blocklist and
+ * benchmark-string removal).  d_out[0, text_bytes) receives d_text[0, text_bytes); then, for every match
+ * m that dach_dev_scan_batch(mode) reports on haystack i, d_out[offs[i] + m.start, offs[i] + m.end) is
+ * set to `fill`.  Bytes outside the haystacks (before offs[0], after offs[n]) are copied unchanged, and
+ * zero-length matches (the empty pattern) mask nothing.  The host form writes out[0, offs[n]) the same way.
+ * Modes, offsets and refusals are those of dach_dev_count_batch (DACH_MATCH_KIND_MISMATCH, DACH_CUDA_ERROR
+ * without a device; no capacity, no DACH_OUTPUT_OVERFLOW); bad offsets leave d_out as it was.
+ * DACH_INVALID_ARGUMENT before anything runs: d_out overlaps [d_text, d_text + text_bytes) (a span reaches
+ * back over bytes another lane may not have read yet, so masking in place is not supported), or a charwise
+ * automaton and fill >= 0x80 (valid UTF-8 stays valid: spans start and end on char boundaries).  A span never
+ * reaches before its haystack's first byte, whatever lengths a deserialized automaton carries.  The calls
+ * synchronise `stream`.  The host form uses the slices of dach_scan_batch_host and copies each slice's masked
+ * bytes back (dach_dev_last_d2h_bytes).  Options kernel and the fallbacks as dach_dev_count_batch; stream
+ * chunks, jobs and shard groups have no mask form. */
+int dach_dev_mask_batch(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                        uint64_t text_bytes, uint8_t fill, uint8_t *d_out, void *stream);
+int dach_mask_batch_host(dach_dev *dev, int mode, const uint8_t *text, const uint64_t *offs, uint64_t n,
+                         uint8_t fill, uint8_t *out);
+
 /* ---- asynchronous scans (jobs) ----------------------------------------------------------
  *
  * dach_dev_scan_batch is one call that synchronises its stream and serialises per handle.  A job is

@@ -95,6 +95,12 @@ extern "C" {
                              text_bytes: u64, d_df: *mut u64, n_df: u64, total: *mut u64, stream: *mut c_void) -> i32;
     /// Windows and re-scans (windows that overflowed option df_pairs) of the handle's last DF call.
     pub fn dach_dev_last_df_windows(dev: *const DachDev, windows: *mut u64, rescans: *mut u64) -> i32;
+    /// The text with every byte a match of iterator `mode` covers set to `fill`; bytes outside the haystacks copied.
+    /// `out` must not overlap the text; a charwise automaton needs fill < 0x80.
+    pub fn dach_mask_batch_host(dev: *mut DachDev, mode: i32, text: *const u8, offs: *const u64, n: u64, fill: u8,
+                                out: *mut u8) -> i32;
+    pub fn dach_dev_mask_batch(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                               text_bytes: u64, fill: u8, d_out: *mut u8, stream: *mut c_void) -> i32;
     /// Device-resident buffers.
     pub fn dach_dev_scan_batch(dev: *mut DachDev, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64,
                                text_bytes: u64, d_out: *mut DachMatch, out_cap: u64, d_out_offs: *mut u64,

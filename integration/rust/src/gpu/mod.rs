@@ -88,6 +88,26 @@ fn scan<P: AsRef<[u8]>>(dev: &Device, mode: i32, haystacks: &[P]) -> Result<Batc
     }
 }
 
+/// Every haystack with the bytes its matches cover set to `fill` (`dach_mask_batch_host`), one output per haystack.
+fn mask<P: AsRef<[u8]>>(dev: &Device, mode: i32, haystacks: &[P], fill: u8) -> Result<Vec<Vec<u8>>, GpuError> {
+    let mut text = Vec::new();
+    let mut offs = Vec::with_capacity(haystacks.len() + 1);
+    offs.push(0u64);
+    for h in haystacks {
+        text.extend_from_slice(h.as_ref());
+        offs.push(text.len() as u64);
+    }
+    let mut out = vec![0u8; text.len()];
+    let rc = unsafe {
+        ffi::dach_mask_batch_host(dev.dev, mode, text.as_ptr(), offs.as_ptr(), haystacks.len() as u64, fill, out.as_mut_ptr())
+    };
+    if rc == ffi::DACH_MATCH_KIND_MISMATCH {
+        panic!("Error: match_kind mismatch"); // src/bytewise.rs:194-197
+    }
+    check(rc)?;
+    Ok(offs.windows(2).map(|w| out[w[0] as usize..w[1] as usize].to_vec()).collect())
+}
+
 /// Drop-in for `daachorse::DoubleArrayAhoCorasick<u32>`: same constructors, same iterator methods, same
 /// `MatchKind` gating -- `use daachorse::gpu::DoubleArrayAhoCorasick;` is the whole switch.  Construction runs the
 /// crate's own builder (src/bytewise/builder.rs) on the host; the serialized automaton crosses the FFI once.
@@ -172,6 +192,19 @@ impl DoubleArrayAhoCorasick {
         assert!(self.match_kind().is_leftmost(), "Error: match_kind must be leftmost.");
         scan(&self.dev, ffi::DACH_LEFTMOST_FIND, h)
     }
+
+    /// Every haystack with the bytes the matches of iterator `mode` cover set to `fill`; no match list.
+    pub fn mask_batch<P: AsRef<[u8]>>(&self, mode: i32, h: &[P], fill: u8) -> Result<Vec<Vec<u8>>, GpuError> {
+        mask(&self.dev, mode, h, fill)
+    }
+    /// `d_text[0..text_bytes)` into `d_out` with every byte a match of iterator `mode` covers set to `fill`, as
+    /// `dach_dev_mask_batch` documents; no match list.
+    /// # Safety
+    /// All pointers are device pointers of the sizes `dach_dev_mask_batch` documents; `d_out` does not overlap the text.
+    pub unsafe fn mask_batch_device(&self, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64, text_bytes: u64, fill: u8,
+                                    d_out: *mut u8, stream: *mut core::ffi::c_void) -> Result<(), GpuError> {
+        check(ffi::dach_dev_mask_batch(self.dev.dev, mode, d_text, d_offs, n, text_bytes, fill, d_out, stream))
+    }
 }
 
 /// Drop-in for `daachorse::CharwiseDoubleArrayAhoCorasick<u32>` (haystacks are `&str`: valid UTF-8).
@@ -242,6 +275,21 @@ impl CharwiseDoubleArrayAhoCorasick {
     pub fn leftmost_find_batch(&self, h: &[&str]) -> Result<BatchMatches, GpuError> {
         assert!(self.match_kind().is_leftmost(), "Error: match_kind must be leftmost.");
         scan(&self.dev, ffi::DACH_LEFTMOST_FIND, h)
+    }
+    /// Every haystack with the chars the matches of iterator `mode` cover set to `fill`, one byte per byte they took;
+    /// `fill` must be ASCII (the library refuses anything else), so the results stay valid UTF-8.
+    pub fn mask_batch(&self, mode: i32, h: &[&str], fill: u8) -> Result<Vec<String>, GpuError> {
+        Ok(mask(&self.dev, mode, h, fill)?
+            .into_iter()
+            .map(|v| String::from_utf8(v).expect("spans start and end on char boundaries"))
+            .collect())
+    }
+    /// As `DoubleArrayAhoCorasick::mask_batch_device`; `fill` must be ASCII.
+    /// # Safety
+    /// All pointers are device pointers of the sizes `dach_dev_mask_batch` documents; `d_out` does not overlap the text.
+    pub unsafe fn mask_batch_device(&self, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64, text_bytes: u64, fill: u8,
+                                    d_out: *mut u8, stream: *mut core::ffi::c_void) -> Result<(), GpuError> {
+        check(ffi::dach_dev_mask_batch(self.dev.dev, mode, d_text, d_offs, n, text_bytes, fill, d_out, stream))
     }
 }
 

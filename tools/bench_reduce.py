@@ -5,6 +5,7 @@
     python tools/bench_reduce.py --output first  ...
     python tools/bench_reduce.py --output hist [--key value|output] ...
     python tools/bench_reduce.py --output df [--key value|output] ...
+    python tools/bench_reduce.py --output mask [--fill N] [--alt-mib M] ...
     python tools/bench_reduce.py --stream --output counts|hist [--key value|output] [--config C2|C3|C3-find] ...
 
 One step = one dach_dev_count_batch / dach_dev_first_batch / dach_dev_hist_batch / dach_dev_df_batch on the step's
@@ -30,6 +31,10 @@ batch (the batches, automata and seeds of bench.py).  One JSON line, bench.py's 
                      carried from step to step.  GB/s by CUDA events around whole steps of the stream form
                      (dach_dev_count_stream / dach_dev_hist_stream) and of scan_stream_device + torch on the same
                      rounds; parity: counts / histogram and the carried state, stream form vs matches stream
+  alternatives       (mask) in the same run: the mask call, COUNT (the same scan without the stores), the copy kernel
+                     alone (a mask call with no haystack), and the matches path + a torch span fill in slices of
+                     --alt-mib; the mask parity checks the host form on the oracle sample's spans, and the whole step
+                     against the torch span fill
   launches_per_step  kernels launched per step
 Nothing is written to the tree.
 """
@@ -113,6 +118,8 @@ def run_reduce_output(args, W, pma, batches, dmode, omode, n, hay_len, step_byte
         return run_stream_output(args, W, pma, batches, dmode, n, hay_len, step_bytes, resident, dev, setup_s)
     if args.output == "df":
         return run_df_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s)
+    if args.output == "mask":
+        return run_mask_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s)
     if args.output == "hist":
         return run_hist_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s)
     counts_t = torch.empty(n, dtype=torch.int64, device=dev)
@@ -582,9 +589,141 @@ def run_df_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, r
     }
 
 
+def torch_span_fill(pma, dmode, t, o, fill, out, slice_haystacks, cap):
+    """The matches path plus torch: every slice of `slice_haystacks` haystacks scanned into a match list, its spans
+    turned into a byte mask (a difference array and a cumsum) and filled into `out`, a copy of the text."""
+    import torch
+
+    out.copy_(t)
+    n = o.numel() - 1
+    out_m = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+    for a in range(0, n, slice_haystacks):
+        b = min(n, a + slice_haystacks)
+        lo, hi = int(o[a]), int(o[b])
+        os_ = o[a:b + 1] - lo
+        r = pma.scan_batch_device(dmode, t[lo:hi], os_, out=out_m)
+        m = r.matches.long()
+        hay = torch.repeat_interleave(torch.arange(b - a, device=t.device), torch.diff(r.offsets))
+        s, e = os_[hay] + m[:, 0], os_[hay] + m[:, 1]
+        d = torch.zeros(hi - lo + 1, dtype=torch.int32, device=t.device)
+        d.index_add_(0, s, torch.ones_like(s, dtype=torch.int32))
+        d.index_add_(0, e, torch.full_like(e, -1, dtype=torch.int32))
+        out[lo:hi].masked_fill_(torch.cumsum(d[:-1], 0) > 0, fill)
+    return out
+
+
+def run_mask_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes, resident, dev, setup_s):
+    """--output mask: every step is one dach_dev_mask_batch on the step's batch.  The same run times, by CUDA events
+    around whole steps on the same batches: COUNT (the same scan without the stores), the copy kernel alone (a mask call
+    with no haystack), and the matches path plus a torch span fill in slices of --alt-mib."""
+    import torch
+
+    fill = args.fill
+    masked = torch.empty(step_bytes, dtype=torch.uint8, device=dev)
+    alt = torch.empty(step_bytes, dtype=torch.uint8, device=dev)
+    counts_t = torch.empty(n, dtype=torch.int64, device=dev)
+    slice_h = max(1, (args.alt_mib << 20) // hay_len)
+    t0_, o0_ = batches[0]
+    r0 = pma.scan_batch_device(dmode, t0_[: int(o0_[min(n, slice_h)])], o0_[: min(n, slice_h) + 1])
+    cap = int(max(r0.matches.shape[0], 1) * 1.25) + 1024
+    del r0
+
+    def mask_step(s):
+        t, o = batches[s % len(batches)]
+        pma.mask_batch_device(dmode, t, o, fill=fill, out=masked[: t.numel()])
+        st = pma.stats()
+        return st["scan_kernel_ms"], st["total_ms"]
+
+    def count_step(s):
+        t, o = batches[s % len(batches)]
+        pma.count_batch_device(dmode, t, o, out=counts_t)
+
+    def copy_step(s):
+        t, o = batches[s % len(batches)]
+        pma.mask_batch_device(dmode, t, o[:1], fill=fill, out=masked[: t.numel()])
+
+    def torch_step(s):
+        t, o = batches[s % len(batches)]
+        torch_span_fill(pma, dmode, t, o, fill, alt[: t.numel()], slice_h, cap)
+
+    def timed(fn):
+        """ms per step over args.steps steps after args.warmup, the steps' results, and the kernels they launched"""
+        for s in range(args.warmup):
+            fn(s)
+        torch.cuda.synchronize()
+        l0 = pma.stats()["launches"]
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+        res = [fn(args.warmup + s) for s in range(args.steps)]
+        ev1.record()
+        torch.cuda.synchronize()
+        return ev0.elapsed_time(ev1) / args.steps, res, pma.stats()["launches"] - l0
+
+    sampler = ClockSampler(dev.index)
+    sampler.start()
+    time.sleep(0.2)
+    n_before = len(sampler.rows)
+    mask_ms, times, launches = timed(mask_step)
+    count_ms, _, _ = timed(count_step)
+    copy_ms, _, _ = timed(copy_step)
+    torch_ms, _, _ = timed(torch_step)
+    time.sleep(0.25)
+    clocks = sampler.stop(skip=n_before)
+    k_ms = float(np.mean([t[0] for t in times]))
+    dev_ms = float(np.mean([t[1] for t in times]))
+    gbs = lambda ms: step_bytes / (ms * 1e-3) / 1e9  # noqa: E731
+    # the whole last step against the torch span fill of the same batch
+    last_batch = (args.warmup + args.steps - 1) % len(batches)
+    t_last, o_last = batches[last_batch]
+    one = pma.mask_batch_device(dmode, t_last, o_last, fill=fill, out=masked[: t_last.numel()])
+    ref = torch_span_fill(pma, dmode, t_last, o_last, fill, alt[: t_last.numel()], slice_h, cap)
+    step_ok = bool(torch.equal(one, ref))
+    masked_bytes = int((one != t_last).sum().item())
+    parity = None
+    if not args.no_cpu:
+        import oracle_api as O
+        import emu_mask_api as EM
+
+        threads = O.cpu_budget()["threads"]
+        ns = max(1, min(n, int(n * args.parity_frac)))
+        opma = W.oracle()
+        lo = W.batch_ranges()[last_batch][0]
+        ptext, poffs = W.host_batch(lo, lo + ns)
+        r = opma.scan_batch(omode, ptext, poffs, nthreads=threads, want_matches=True)
+        want = EM.expected_from_matches(ptext, poffs, r["matches"], r["counts"], fill)
+        got = pma.mask_batch_host(dmode, ptext, poffs, fill=fill)
+        parity = {"mask_equal": bool(np.array_equal(got, want)), "haystacks_checked": ns, "share_of_batch": ns / n,
+                  "what": "host mask of the first %d haystacks of the last batch vs the oracle's matches turned into spans" % ns}
+    parity = dict(parity or {}, step_equals_torch_span_fill=step_ok)
+    peak, peak_src = measured_peaks()
+    achieved = step_bytes / (k_ms * 1e-3) / 1e9
+    roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
+                "kernel": "k_scan_machine_rk (mask)", "kernel_ms": k_ms, "algorithmic_bytes_per_launch": step_bytes,
+                "peak_source": peak_src,
+                "note": "algorithmic bytes = 1 B read per haystack byte offered; kernel_ms = mean CUDA-event time of the scan kernel"}
+    return {
+        "metric": metric_name(W.spec) + ", mask", "output": "mask", "value": gbs(dev_ms), "unit": UNIT,
+        "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": mask_ms, "device_ms_per_step": dev_ms,
+        "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
+        "config": {"workload": "%s: %s, %s, %d haystacks x %d B per step, %d batch(es) resident (%.2f GiB)" % (
+                       args.config, W.spec["what"], W.mode_name, n, hay_len, len(batches), resident / 2**30),
+                   "n_patterns": len(W.ps), "hay_len": hay_len, "bytes_per_gpu": step_bytes, "options": args.option,
+                   "setup_s": setup_s, "fill": fill, "alt_mib": args.alt_mib},
+        "masked_bytes_last_step": masked_bytes,
+        "alternatives": {"unit": UNIT, "what": "CUDA events around %d whole steps each, same batches" % args.steps,
+                         "mask": gbs(mask_ms), "count": gbs(count_ms), "copy_only": gbs(copy_ms),
+                         "matches_plus_torch_fill": gbs(torch_ms), "mask_ms": mask_ms, "count_ms": count_ms,
+                         "copy_ms": copy_ms, "matches_plus_torch_fill_ms": torch_ms},
+        "card": _card(), "roofline": roofline, "parity": parity,
+        "gpu_launches": int(launches), "launches_per_step": launches / args.steps, "clocks": clocks,
+    }
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--output", required=True, choices=["counts", "first", "hist", "df"])
+    ap.add_argument("--output", required=True, choices=["counts", "first", "hist", "df", "mask"])
+    ap.add_argument("--fill", type=int, default=ord("*"), help="--output mask: the fill byte")
+    ap.add_argument("--alt-mib", type=int, default=256, help="--output mask: slice of the matches-plus-torch baseline")
     ap.add_argument("--stream", action="store_true", help="--output counts / hist on stream chunks: one round per step")
     ap.add_argument("--key", default="value", choices=["value", "output"], help="--output hist / df: key")
     ap.add_argument("--config", default="C3", choices=sorted(CONFIGS))

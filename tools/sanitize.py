@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 import daachorse_b200 as D
+import emu_mask_api as EM
 import oracle_api as O
 from daachorse_b200 import shard
 
@@ -214,6 +215,35 @@ def doc_frequencies():
                 n_scans += 1
 
 
+def masked_text():
+    """dach_mask_batch_host / dach_dev_mask_batch on every machine that serves them (StdMachine3 with and without
+    segments, LmMachine, CwMachine, the lane-per-haystack loops); against the oracle's matches turned into spans, and
+    the device form's output at an odd offset from its text."""
+    global n_scans
+    dev = torch.device("cuda", 0)
+    for cw in (False, True):
+        for kind in (0, 1):
+            pma, opma, text, offs = random_case(80 + 10 * kind + cw, cw, kind)
+            for mode in ([D.LEFTMOST_FIND] if kind else [D.FIND, D.FIND_OVERLAPPING, D.FIND_OVERLAPPING_NO_SUFFIX]):
+                ref = opma.scan_batch(ORC[mode], text, offs, want_matches=True)
+                want = EM.expected_from_matches(text, offs, ref["matches"], ref["counts"], 0x2A)
+                for opts in ({"kernel": 3}, {"kernel": 3, "seg_len": 64}, {"kernel": 0}):
+                    for k, v in opts.items():
+                        pma.set_option(k, v)
+                    assert np.array_equal(pma.mask_batch_host(mode, text, offs), want), (cw, kind, mode, opts)
+                    n_scans += 1
+                    pma.set_option("seg_len", 0)
+                pma.set_option("kernel", 3)
+                pad = 3
+                buf = torch.empty(text.size + pad, dtype=torch.uint8, device=dev)
+                buf[pad:] = torch.from_numpy(text.copy()).to(dev)
+                out = torch.empty(text.size + 7, dtype=torch.uint8, device=dev)
+                o = torch.from_numpy(offs.astype(np.int64)).to(dev)
+                pma.mask_batch_device(mode, buf[pad:], o, out=out[7:])
+                assert np.array_equal(out[7:].cpu().numpy(), want)
+                n_scans += 1
+
+
 def streams_jobs_groups():
     global n_scans
     dev = torch.device("cuda", 0)
@@ -287,6 +317,7 @@ if __name__ == "__main__":
     counts_and_first()
     histograms()
     doc_frequencies()
+    masked_text()
     streams_jobs_groups()
     torch.cuda.synchronize()
     print("sanitize.py: %d scans, all equal to the oracle" % n_scans)
