@@ -20,9 +20,16 @@ device the scan methods raise DaachorseError(CUDA_ERROR).
 The crate's iterators are lazy; here an iterator call scans the haystack eagerly on the
 device and then yields the same Match sequence.  The ``*_batch`` methods are the
 throughput interface (many haystacks per call).
+
+Streams: every ``*_device`` form takes ``stream=`` -- ``None`` (the current stream of the text's
+device), a torch stream, or a raw ``cudaStream_t`` handle (int).  A stream other than the current
+one is made to wait for the work queued so far on the current stream before each library call, so
+the inputs written there and the outputs the wrapper allocates there are ready; the call
+synchronises its stream before it returns, so its results may be used on the current stream.
 """
 import ctypes as C
 import enum
+import threading
 
 import numpy as np
 
@@ -128,6 +135,46 @@ def _ptr(a):
     return C.c_void_p(a.ctypes.data) if a.size else None
 
 
+def _stream_handle(stream, device):
+    """The raw cudaStream_t of ``stream``: None = the current stream of ``device``, a torch stream, or a handle."""
+    import torch
+
+    if stream is None:
+        return torch.cuda.current_stream(device).cuda_stream
+    return int(stream.cuda_stream) if hasattr(stream, "cuda_stream") else int(stream)
+
+
+def _wait_stream(handle, current, device):
+    """Stream ``handle`` waits for the work queued so far on ``current``."""
+    import torch
+
+    torch.cuda.ExternalStream(handle, device=device).wait_stream(current)
+
+
+def _ordered_stream(stream, device):
+    """``stream`` as a ctypes handle, ordered after the current stream of ``device`` when it is another stream: the
+    wrappers allocate and fill on the current stream, and the caller's inputs were written there.  Called right
+    before every library call, retries included.  The same stream costs nothing."""
+    import torch
+
+    handle = _stream_handle(stream, device)
+    current = torch.cuda.current_stream(device)
+    if handle != current.cuda_stream:
+        _wait_stream(handle, current, device)
+    return C.c_void_p(handle)
+
+
+def _torch_stream(stream, device):
+    """``stream`` (None, a torch stream or a raw handle) as a torch stream object, for ``record_stream``."""
+    import torch
+
+    if stream is None:
+        return torch.cuda.current_stream(device)
+    if isinstance(stream, torch.cuda.Stream):
+        return stream
+    return torch.cuda.ExternalStream(_stream_handle(stream, device), device=device)
+
+
 class _Automaton:
     """Shared implementation of the two automaton classes."""
 
@@ -136,6 +183,7 @@ class _Automaton:
     def __init__(self, handle):
         self._h = handle
         self._devs = {}
+        self._devs_lock = threading.Lock()  # one upload per device, whichever thread calls first
 
     # -- construction ----------------------------------------------------------------------
     @classmethod
@@ -238,15 +286,17 @@ class _Automaton:
 
     # -- device ---------------------------------------------------------------------------------
     def device_handle(self, device=None):
-        """Uploads the scan image to ``device`` once (default: the current CUDA device)."""
+        """Uploads the scan image to ``device`` once (default: the current CUDA device), also when several host
+        threads make their first call at the same time: they all get the one handle."""
         L = _lib.load()
         if device is None:
             device = _current_device()
-        d = self._devs.get(device)
-        if d is None:
-            d = C.c_void_p()
-            _check(L.dach_dev_upload(self._h, int(device), C.byref(d)))
-            self._devs[device] = d
+        with self._devs_lock:
+            d = self._devs.get(device)
+            if d is None:
+                d = C.c_void_p()
+                _check(L.dach_dev_upload(self._h, int(device), C.byref(d)))
+                self._devs[device] = d
         return d
 
     def set_option(self, name, value, device=None):
@@ -306,7 +356,9 @@ class _Automaton:
     def scan_batch_device(self, mode, text, offs, out=None, out_offs=None, stream=None):
         """Device-resident scan.  ``text`` (uint8) and ``offs`` (int64/uint64, n+1) are CUDA torch
         tensors; returns BatchResult with an (total, 3) int32-typed view of u32 triples and an
-        int64 offsets tensor, both on the device.  ``out``: optional preallocated (cap, 3) int32."""
+        int64 offsets tensor, both on the device.  ``out``: optional preallocated (cap, 3) int32.  ``stream``: None, a
+        torch stream or a raw handle; another stream than the current one is ordered after the current one (module
+        docstring), and the call synchronises it before it returns."""
         import torch
 
         self._assert_mode(mode)
@@ -318,14 +370,13 @@ class _Automaton:
         if out_offs is None:
             out_offs = torch.empty(n + 1, dtype=torch.int64, device=text.device)
         cap = out.shape[0] if out is not None else max(1024, int(text.numel() // 8))
-        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
         while True:
             if out is None or out.shape[0] < cap:
                 out = torch.empty((cap, 3), dtype=torch.int32, device=text.device)
             need = C.c_uint64()
             rc = L.dach_dev_scan_batch(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n,
                                        text.numel(), C.c_void_p(out.data_ptr()), out.shape[0],
-                                       C.c_void_p(out_offs.data_ptr()), C.byref(need), st)
+                                       C.c_void_p(out_offs.data_ptr()), C.byref(need), _ordered_stream(stream, text.device))
             if rc == _lib.OUTPUT_OVERFLOW:
                 if int(need.value) <= cap:
                     raise DaachorseError(rc, "overflow reported although capacity %d >= needed %d" % (cap, need.value))
@@ -340,7 +391,9 @@ class _Automaton:
         (src/bytewise.rs:627-729): haystack i is the next chunk of stream i.  ``state`` (CUDA int32/uint32,
         n entries) holds each stream's state id and is updated in place; ``pos`` (optional, n entries) is
         the stream position of each chunk's first byte and is added to the reported positions.  For every
-        byte: consume(byte), then matches().  Returns a BatchResult of device tensors."""
+        byte: consume(byte), then matches().  Returns a BatchResult of device tensors.  ``stream`` as in
+        ``scan_batch_device``: the copy of ``state`` an overflow retry restarts from is taken on the current stream,
+        before the call."""
         import torch
 
         self._assert_mode(mode)
@@ -352,7 +405,6 @@ class _Automaton:
         if out_offs is None:
             out_offs = torch.empty(n + 1, dtype=torch.int64, device=text.device)
         cap = out.shape[0] if out is not None else max(1024, int(text.numel() // 8))
-        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
         state_in = state.clone()  # the call advances `state` even when the output overflows
         while True:
             if out is None or out.shape[0] < cap:
@@ -361,7 +413,7 @@ class _Automaton:
             rc = L.dach_dev_scan_stream(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
                                         C.c_void_p(state.data_ptr()), C.c_void_p(pos.data_ptr()) if pos is not None else None,
                                         C.c_void_p(out.data_ptr()), out.shape[0], C.c_void_p(out_offs.data_ptr()),
-                                        C.byref(need), st)
+                                        C.byref(need), _ordered_stream(stream, text.device))
             if rc == _lib.OUTPUT_OVERFLOW:
                 if int(need.value) <= cap:
                     raise DaachorseError(rc, "overflow reported although capacity %d >= needed %d" % (cap, need.value))
@@ -382,12 +434,6 @@ class _Automaton:
         dev = text.device.index if text.device.index is not None else torch.cuda.current_device()
         return dev, self.device_handle(dev)
 
-    @staticmethod
-    def _stream_ptr(stream, text):
-        import torch
-
-        return C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
-
     def count_stream_device(self, mode, text, offs, state, out=None, stream=None):
         """Matches per chunk of ``scan_stream_device`` without the matches: an int64 CUDA tensor of n counts
         (``out``: optional preallocated one), ``state`` advanced in place."""
@@ -401,7 +447,7 @@ class _Automaton:
         total = C.c_uint64()
         _check(_lib.load().dach_dev_count_stream(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
                                                  C.c_void_p(state.data_ptr()), C.c_void_p(out.data_ptr()), C.byref(total),
-                                                 self._stream_ptr(stream, text)))
+                                                 _ordered_stream(stream, text.device)))
         return out
 
     def first_stream_device(self, mode, text, offs, state, pos=None, out=None, found=None, stream=None):
@@ -421,7 +467,7 @@ class _Automaton:
         _check(_lib.load().dach_dev_first_stream(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
                                                  C.c_void_p(state.data_ptr()), C.c_void_p(pos.data_ptr()) if pos is not None else None,
                                                  C.c_void_p(out.data_ptr()), C.c_void_p(found.data_ptr()), C.byref(nf),
-                                                 self._stream_ptr(stream, text)))
+                                                 _ordered_stream(stream, text.device)))
         return out, found
 
     def pattern_counts_stream_device(self, mode, text, offs, state, key="value", out=None, stream=None):
@@ -439,7 +485,7 @@ class _Automaton:
         _check(_lib.load().dach_dev_hist_stream(d, mode, HIST_KEYS[key], C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()),
                                                 offs.numel() - 1, text.numel(), C.c_void_p(state.data_ptr()),
                                                 C.c_void_p(out.data_ptr()), out.numel(), C.byref(total),
-                                                self._stream_ptr(stream, text)))
+                                                _ordered_stream(stream, text.device)))
         return out
 
     # -- counts and first matches (no match list) -------------------------------------------------
@@ -487,10 +533,9 @@ class _Automaton:
             out = torch.empty(n, dtype=torch.int64, device=text.device)
         _check_device_batch(text, offs, dev, counts=out)
         d = self.device_handle(dev)
-        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
         total = C.c_uint64()
         _check(_lib.load().dach_dev_count_batch(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
-                                                C.c_void_p(out.data_ptr()), C.byref(total), st))
+                                                C.c_void_p(out.data_ptr()), C.byref(total), _ordered_stream(stream, text.device)))
         return out
 
     def first_batch_device(self, mode, text, offs, out=None, found=None, stream=None):
@@ -507,10 +552,9 @@ class _Automaton:
             found = torch.empty(n, dtype=torch.bool, device=text.device)
         _check_device_batch(text, offs, dev, first=out, found=found)
         d = self.device_handle(dev)
-        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
         nf = C.c_uint64()
         _check(_lib.load().dach_dev_first_batch(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), n, text.numel(),
-                                                C.c_void_p(out.data_ptr()), C.c_void_p(found.data_ptr()), C.byref(nf), st))
+                                                C.c_void_p(out.data_ptr()), C.c_void_p(found.data_ptr()), C.byref(nf), _ordered_stream(stream, text.device)))
         return out, found
 
     def pattern_counts_host(self, mode, text, offs, key="value", out=None, device=None):
@@ -543,11 +587,10 @@ class _Automaton:
             out = torch.zeros(need, dtype=torch.int64, device=text.device)
         _check_device_batch(text, offs, dev, hist=out, hist_len=need)
         d = self.device_handle(dev)
-        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
         total = C.c_uint64()
         _check(_lib.load().dach_dev_hist_batch(d, mode, HIST_KEYS[key], C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()),
                                                offs.numel() - 1, text.numel(), C.c_void_p(out.data_ptr()), out.numel(),
-                                               C.byref(total), st))
+                                               C.byref(total), _ordered_stream(stream, text.device)))
         return out
 
     def doc_counts_host(self, mode, text, offs, key="value", out=None, device=None):
@@ -580,11 +623,10 @@ class _Automaton:
             out = torch.zeros(need, dtype=torch.int64, device=text.device)
         _check_device_batch(text, offs, dev, hist=out, hist_len=need)
         d = self.device_handle(dev)
-        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
         total = C.c_uint64()
         _check(_lib.load().dach_dev_df_batch(d, mode, HIST_KEYS[key], C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()),
                                              offs.numel() - 1, text.numel(), C.c_void_p(out.data_ptr()), out.numel(),
-                                             C.byref(total), st))
+                                             C.byref(total), _ordered_stream(stream, text.device)))
         return out
 
     def last_doc_windows(self, device=None):
@@ -636,9 +678,8 @@ class _Automaton:
             out = torch.empty(text.numel(), dtype=torch.uint8, device=text.device)
         _check_device_batch(text, offs, dev, masked=out)
         d = self.device_handle(dev)
-        st = C.c_void_p(stream if stream is not None else torch.cuda.current_stream(text.device).cuda_stream)
         _check(_lib.load().dach_dev_mask_batch(d, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()), offs.numel() - 1,
-                                               text.numel(), fill, C.c_void_p(out.data_ptr()), st))
+                                               text.numel(), fill, C.c_void_p(out.data_ptr()), _ordered_stream(stream, text.device)))
         return out
 
     def mask_batch(self, haystacks, fill=b"*", mode=None):
@@ -730,7 +771,9 @@ class _Automaton:
 
 
 class Job:
-    """dach_job: one in-flight scan of device-resident buffers (include/daachorse_b200.h, "asynchronous scans")."""
+    """dach_job: one in-flight scan of device-resident buffers (include/daachorse_b200.h, "asynchronous scans").
+    ``scan`` and ``place`` only enqueue work and keep the tensors they are given alive in stream order; inputs written
+    on another stream than the one they are enqueued on must be ordered by the caller first."""
 
     def __init__(self, pma, device=None):
         import torch
@@ -755,23 +798,37 @@ class Job:
         return C.c_void_p(stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream))
 
     def scan(self, mode, text, offs, cap_matches, stream=None):
-        """Enqueue the scan of ``text`` (uint8 CUDA tensor) / ``offs`` (int64, n+1) on ``stream``."""
+        """Enqueue the scan of ``text`` (uint8 CUDA tensor) / ``offs`` (int64, n+1) on ``stream`` (None, a torch
+        stream or a raw handle).  The next ``scan`` may be enqueued before ``wait``, and the caller may drop its
+        references at once: both tensors are recorded on ``stream`` (``record_stream``), so the caching allocator
+        hands their memory out again only after the scan has read it.  Unlike the ``*_device`` forms this does not
+        wait for the current stream: as with torch's own streams, inputs written on another stream are the caller's to
+        order (``stream.wait_stream(...)``)."""
         self._pma._assert_mode(mode)
         _check_device_batch(text, offs, self._dev)
+        ts = _torch_stream(stream, text.device)
+        text.record_stream(ts)
+        offs.record_stream(ts)
         self._keep = (text, offs)  # the kernels read them after this call returns
         _check(_lib.load().dach_job_scan(self._h, mode, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()),
-                                         offs.numel() - 1, text.numel(), int(cap_matches), self._stream(stream, text.device)))
+                                         offs.numel() - 1, text.numel(), int(cap_matches), C.c_void_p(ts.cuda_stream)))
 
     def place(self, out, out_offs, base=None, stream=None):
         """Enqueue the gather into ``out`` ((cap, 3) int32) / ``out_offs`` (int64, n+1); ``base``: optional
-        1-element int64 CUDA tensor, index of the first match in ``out``."""
+        1-element int64 CUDA tensor, index of the first match in ``out``.  ``out``, ``out_offs`` and ``base`` are
+        recorded on ``stream`` as ``scan`` records its inputs; ``base``, too, is the caller's to order if it was
+        written on another stream."""
         _check_device_batch(self._keep[0], self._keep[1], out.device.index, out, out_offs)
         if base is not None and (not base.is_cuda or base.dtype not in (torch_int64(),) or base.numel() < 1):
             raise DaachorseError(_lib.INVALID_ARGUMENT, "base must be a 1-element int64 CUDA tensor")
+        ts = _torch_stream(stream, out.device)
+        for t in (out, out_offs, base):
+            if t is not None:
+                t.record_stream(ts)
         self._out = (out, out_offs, base)
         _check(_lib.load().dach_job_place(self._h, C.c_void_p(out.data_ptr()), out.shape[0], C.c_void_p(out_offs.data_ptr()),
                                           C.c_void_p(base.data_ptr()) if base is not None else None,
-                                          self._stream(stream, out.device)))
+                                          C.c_void_p(ts.cuda_stream)))
 
     def wait(self):
         """Block until the placement is done; returns the number of matches (raises on overflow)."""
