@@ -24,7 +24,8 @@ SYMBOLS = [
     "dach_dev_mask_batch", "dach_mask_batch_host", "dach_dev_kernel_launches", "dach_dev_last_scan_kernel_ms",
     "dach_dev_last_total_ms", "dach_dev_last_h2d_bytes", "dach_dev_last_d2h_bytes",
     "dach_dev_set_option", "dach_last_error", "dach_abi_version",
-    "dach_job_create", "dach_job_free", "dach_job_scan", "dach_job_place", "dach_job_wait", "dach_job_scan_kernel_ms", "dach_job_push_ms", "dach_job_times",
+    "dach_job_create", "dach_job_free", "dach_job_scan", "dach_job_place", "dach_job_count", "dach_job_first",
+    "dach_job_hist", "dach_job_mask", "dach_job_wait", "dach_job_scan_kernel_ms", "dach_job_push_ms", "dach_job_times",
     "dach_group_create", "dach_group_export", "dach_group_connect", "dach_group_place", "dach_group_finish",
     "dach_group_result", "dach_group_free",
 ]
@@ -117,6 +118,10 @@ def load():
     L.dach_job_free.restype = None
     L.dach_job_scan.argtypes = [vp, C.c_int, vp, vp, u64, u64, u64, vp]
     L.dach_job_place.argtypes = [vp, vp, u64, vp, vp, vp]
+    L.dach_job_count.argtypes = [vp, C.c_int, vp, vp, u64, u64, vp, vp]
+    L.dach_job_first.argtypes = [vp, C.c_int, vp, vp, u64, u64, vp, vp, vp]
+    L.dach_job_hist.argtypes = [vp, C.c_int, C.c_int, vp, vp, u64, u64, vp, u64, vp]
+    L.dach_job_mask.argtypes = [vp, C.c_int, vp, vp, u64, u64, C.c_uint8, vp, vp]
     L.dach_job_wait.argtypes = [vp, C.POINTER(u64)]
     L.dach_job_scan_kernel_ms.argtypes = [vp]
     L.dach_job_scan_kernel_ms.restype = C.c_double
@@ -132,7 +137,8 @@ def load():
     L.dach_group_result.argtypes = [vp, pp, pp]
     L.dach_group_free.argtypes = [vp]
     L.dach_group_free.restype = None
-    for name in ("dach_job_create", "dach_job_scan", "dach_job_place", "dach_job_wait", "dach_group_create", "dach_group_export",
+    for name in ("dach_job_create", "dach_job_scan", "dach_job_place", "dach_job_count", "dach_job_first", "dach_job_hist",
+                 "dach_job_mask", "dach_job_wait", "dach_group_create", "dach_group_export",
                  "dach_group_connect", "dach_group_place", "dach_group_finish", "dach_group_result"):
         getattr(L, name).restype = C.c_int
     if L.dach_abi_version() != 2:

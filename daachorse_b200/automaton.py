@@ -830,8 +830,82 @@ class Job:
                                           C.c_void_p(base.data_ptr()) if base is not None else None,
                                           C.c_void_p(ts.cuda_stream)))
 
+    # -- reductions: count_batch_device ... mask_batch_device on the job ---------------------------------------------
+    # Each enqueues on ``stream`` and returns the output tensors at once; they hold the results once ``wait`` returns or
+    # on ``stream`` after the call.  Inputs and outputs are recorded on ``stream`` as ``scan`` records its inputs, and
+    # inputs written on another stream are the caller's to order.  Outputs the wrapper creates are allocated on
+    # ``stream``, so the histogram's zeros come before the scan with no wait between streams.
+    def _enqueue(self, fn, head, text, offs, tail, ts, tensors):
+        """dach_job_<fn>(job, *head, text, offs, n, text_bytes, *tail, stream) after recording ``tensors`` on ``ts``."""
+        for t in (text, offs) + tensors:
+            t.record_stream(ts)
+        _check(getattr(_lib.load(), "dach_job_" + fn)(self._h, *head, C.c_void_p(text.data_ptr()), C.c_void_p(offs.data_ptr()),
+                                                      offs.numel() - 1, text.numel(), *tail, C.c_void_p(ts.cuda_stream)))
+
+    def count(self, mode, text, offs, out=None, stream=None):
+        """``count_batch_device`` on the job: the int64 counts (``out``: optional preallocated one); ``wait`` returns
+        their sum."""
+        import torch
+
+        self._pma._assert_mode(mode)
+        _check_device_batch(text, offs, self._dev, counts=out)
+        ts = _torch_stream(stream, text.device)
+        if out is None:
+            with torch.cuda.stream(ts):
+                out = torch.empty(offs.numel() - 1, dtype=torch.int64, device=text.device)
+        self._enqueue("count", (mode,), text, offs, (C.c_void_p(out.data_ptr()),), ts, (out,))
+        return out
+
+    def first(self, mode, text, offs, out=None, found=None, stream=None):
+        """``first_batch_device`` on the job: ``(first, found)``; ``wait`` returns the number of haystacks with a match."""
+        import torch
+
+        self._pma._assert_mode(mode)
+        _check_device_batch(text, offs, self._dev, first=out, found=found)
+        ts = _torch_stream(stream, text.device)
+        n = offs.numel() - 1
+        with torch.cuda.stream(ts):
+            if out is None:
+                out = torch.empty((n, 3), dtype=torch.int32, device=text.device)
+            if found is None:
+                found = torch.empty(n, dtype=torch.bool, device=text.device)
+        self._enqueue("first", (mode,), text, offs, (C.c_void_p(out.data_ptr()), C.c_void_p(found.data_ptr())), ts, (out, found))
+        return out, found
+
+    def pattern_counts(self, mode, text, offs, key="value", out=None, stream=None):
+        """``pattern_counts_device`` on the job: the int64 histogram, added into ``out`` if given (zeros otherwise).
+        Jobs may add into one histogram at the same time; ``wait`` returns the number of matches this call added."""
+        import torch
+
+        self._pma._assert_mode(mode)
+        need = self._pma._hist_len(key)
+        _check_device_batch(text, offs, self._dev, hist=out, hist_len=need)
+        ts = _torch_stream(stream, text.device)
+        if out is None:
+            with torch.cuda.stream(ts):
+                out = torch.zeros(need, dtype=torch.int64, device=text.device)
+        self._enqueue("hist", (mode, HIST_KEYS[key]), text, offs, (C.c_void_p(out.data_ptr()), out.numel()), ts, (out,))
+        return out
+
+    def mask(self, mode, text, offs, fill=ord("*"), out=None, stream=None):
+        """``mask_batch_device`` on the job: a uint8 tensor of ``text``'s size (``out``: optional preallocated one, which
+        must not overlap ``text``); ``wait`` returns 0."""
+        import torch
+
+        fill = self._pma._fill_byte(fill)
+        self._pma._assert_mode(mode)
+        _check_device_batch(text, offs, self._dev, masked=out)
+        ts = _torch_stream(stream, text.device)
+        if out is None:
+            with torch.cuda.stream(ts):
+                out = torch.empty(text.numel(), dtype=torch.uint8, device=text.device)
+        self._enqueue("mask", (mode,), text, offs, (fill, C.c_void_p(out.data_ptr())), ts, (out,))
+        return out
+
     def wait(self):
-        """Block until the placement is done; returns the number of matches (raises on overflow)."""
+        """Block until the job's last operation is done.  Returns the number of matches after ``place`` (raises on
+        overflow), the total of the synchronous twin after a reduction (counts' sum, haystacks with a match, matches
+        added into the histogram; 0 for ``mask``); bad offsets raise INVALID_ARGUMENT and leave the outputs as they were."""
         need = C.c_uint64()
         _check(_lib.load().dach_job_wait(self._h, C.byref(need)))
         return int(need.value)

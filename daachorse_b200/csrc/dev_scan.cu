@@ -1339,7 +1339,8 @@ struct dach_dev {
                              // lane-per-haystack kernels
     // stats
     std::atomic<uint64_t> launches{0};
-    cudaEvent_t ev_ref = nullptr;  // time zero of dach_job_times (recorded at the first job scan)
+    cudaEvent_t ev_ref = nullptr;  // time zero of dach_job_times (recorded at the handle's first job operation)
+    std::mutex ev_ref_mu;           // ... set under this lock, not d->mu: a job never waits for a synchronous call
     double last_scan_ms = 0, last_total_ms = 0;
     uint64_t last_h2d = 0, last_d2h = 0;
     // DF (dach_dev_df_batch / dach_df_batch_host, both under mu): the two pair sets, shared by every window of both
@@ -1358,6 +1359,10 @@ struct dach_job {
     dach_dev* d = nullptr;
     Workspace W;
     uint64_t out_cap = ~0ull;  // capacity the placement was given (for the overflow report)
+    // the job's last operation, which dach_job_wait reports: RK_MATCHES (dach_job_scan, then dach_job_place or
+    // dach_group_place), or RK_COUNT / RK_FIRST / RK_HIST / RK_MASK (dach_job_count ... dach_job_mask)
+    int rk = RK_MATCHES;
+    bool unplaced = false;  // a dach_job_scan whose placement has not been enqueued: a reduction may not reuse its buffers
 };
 
 namespace {
@@ -2417,12 +2422,12 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
     return DACH_OK;
 }
 
-// wait for enqueue_rk's work, report
+// wait for enqueue_rk's work, report.  d == nullptr (jobs): the handle's timings are left to its synchronous calls.
 int finish_rk(dach_dev* d, Workspace& W, uint64_t* total) {
     if (!cuda_ok(cudaEventSynchronize(W.ev_placed), "scan pipeline")) return DACH_CUDA_ERROR;
     float ms = 0;
-    if (cudaEventElapsedTime(&ms, W.ev[3], W.ev[1]) == cudaSuccess) d->last_scan_ms = ms;
-    if (cudaEventElapsedTime(&ms, W.ev[0], W.ev[2]) == cudaSuccess) d->last_total_ms = ms;
+    if (d && cudaEventElapsedTime(&ms, W.ev[3], W.ev[1]) == cudaSuccess) d->last_scan_ms = ms;
+    if (d && cudaEventElapsedTime(&ms, W.ev[0], W.ev[2]) == cudaSuccess) d->last_total_ms = ms;
     if (W.pinned->ctrl.bad_offsets) {
         set_error("haystack offsets must be ascending and inside text_bytes, and no haystack may reach 4 GiB (match positions are u32)");
         return DACH_INVALID_ARGUMENT;
@@ -3146,6 +3151,50 @@ int dach_mask_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint6
     return guarded([&]() -> int { return mask_batch_host_impl(d, mode, text, offs, n, fill, out); });
 }
 
+}  // extern "C"
+
+namespace {
+// time zero of dach_job_times: recorded on `stream` by the handle's first job operation
+// (tried again by the next job operation if the event cannot be created)
+void job_time_zero(dach_dev* d, cudaStream_t stream) {
+    std::lock_guard<std::mutex> lk(d->ev_ref_mu);
+    if (d->ev_ref) return;
+    if (cudaEventCreate(&d->ev_ref) == cudaSuccess) cudaEventRecord(d->ev_ref, stream);
+    else d->ev_ref = nullptr;
+}
+
+// COUNT / FIRST / HIST / MASK on a job: the mode check of the synchronous call (the caller has made the others), then
+// enqueue_rk on the job's workspace, ordered after the job's previous operation; dach_job_wait reports it.  No handle
+// mutex and no handle-wide state: the job's own workspace, events and pinned block only.
+int job_rk(dach_job* j, int rk, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+           uint64_t* d_counts, dach_match* d_first, uint8_t* d_found, uint64_t* d_hist, uint8_t* d_masked, uint8_t fill, void* stream) {
+    int rc = check_mode(j->d, mode);
+    if (rc) return rc;
+    if (n > 0xfffffff0ull) {  // enqueue_rk's check, made here so that nothing at all is recorded on the stream
+        set_error("too many haystacks in one batch (max 2^32-16)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    if (j->unplaced) {
+        set_error("the job's scan has not been placed (dach_job_place comes before the job's next operation)");
+        return DACH_INVALID_ARGUMENT;
+    }
+    return guarded([&]() -> int {
+        DeviceGuard g(j->d->device);
+        if (!g.ok) return DACH_CUDA_ERROR;
+        const cudaStream_t st = static_cast<cudaStream_t>(stream);
+        job_time_zero(j->d, st);
+        const int r = enqueue_rk(j->d, j->W, rk, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, d_counts, d_first,
+                                 d_found, st, key, d_hist, nullptr, nullptr, d_masked, fill);
+        if (r) return r;
+        j->W.job_open = true;  // the job's next operation waits for W.ev_placed
+        j->rk = rk;
+        return DACH_OK;
+    });
+}
+}  // namespace
+
+extern "C" {
+
 // ---- asynchronous jobs ------------------------------------------------------------------------------
 
 int dach_job_create(dach_dev* d, dach_job** out) {
@@ -3189,12 +3238,14 @@ int dach_job_scan(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* 
     return guarded([&]() -> int {
         DeviceGuard g(j->d->device);
         if (!g.ok) return DACH_CUDA_ERROR;
-        {
-            std::lock_guard<std::mutex> lk(j->d->mu);
-            if (!j->d->ev_ref && cudaEventCreate(&j->d->ev_ref) == cudaSuccess) cudaEventRecord(j->d->ev_ref, static_cast<cudaStream_t>(stream));
+        job_time_zero(j->d, static_cast<cudaStream_t>(stream));
+        const int r = enqueue_scan(j->d, j->W, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, cap_matches,
+                                   static_cast<cudaStream_t>(stream));
+        if (!r) {
+            j->rk = RK_MATCHES;
+            j->unplaced = true;
         }
-        return enqueue_scan(j->d, j->W, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, cap_matches,
-                            static_cast<cudaStream_t>(stream));
+        return r;
     });
 }
 
@@ -3203,17 +3254,73 @@ int dach_job_place(dach_job* j, dach_match* d_out, uint64_t out_cap, uint64_t* d
         set_error("null argument");
         return DACH_INVALID_ARGUMENT;
     }
+    if (j->rk != RK_MATCHES) {
+        set_error("no scan to place: the job's last operation was a count, first-match, histogram or mask");
+        return DACH_INVALID_ARGUMENT;
+    }
     return guarded([&]() -> int {
         DeviceGuard g(j->d->device);
         if (!g.ok) return DACH_CUDA_ERROR;
         j->out_cap = out_cap;
-        return enqueue_place(j->d, j->W, d_out, out_cap, d_out_offs, reinterpret_cast<const unsigned long long*>(d_base), true,
-                             static_cast<cudaStream_t>(stream));
+        const int r = enqueue_place(j->d, j->W, d_out, out_cap, d_out_offs, reinterpret_cast<const unsigned long long*>(d_base), true,
+                                    static_cast<cudaStream_t>(stream));
+        if (!r) j->unplaced = false;
+        return r;
     });
+}
+
+int dach_job_count(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                   uint64_t* d_counts, void* stream) {
+    if (!j || !d_offs || (n && !d_counts)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    return job_rk(j, RK_COUNT, mode, 0, d_text, d_offs, n, text_bytes, d_counts, nullptr, nullptr, nullptr, nullptr, 0, stream);
+}
+
+int dach_job_first(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                   dach_match* d_first, uint8_t* d_found, void* stream) {
+    if (!j || !d_offs || (n && (!d_first || !d_found))) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    return job_rk(j, RK_FIRST, mode, 0, d_text, d_offs, n, text_bytes, nullptr, d_first, d_found, nullptr, nullptr, 0, stream);
+}
+
+int dach_job_hist(dach_job* j, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+                  uint64_t* d_hist, uint64_t n_hist, void* stream) {
+    if (!j || !d_offs || (n_hist && !d_hist)) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    const int rc = check_hist(j->d, key, n_hist);
+    if (rc) return rc;
+    return job_rk(j, RK_HIST, mode, key, d_text, d_offs, n, text_bytes, nullptr, nullptr, nullptr, d_hist, nullptr, 0, stream);
+}
+
+int dach_job_mask(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes, uint8_t fill,
+                  uint8_t* d_out, void* stream) {
+    if (!j || !d_offs || (text_bytes && (!d_text || !d_out))) {
+        set_error("null argument");
+        return DACH_INVALID_ARGUMENT;
+    }
+    const int rc = check_mask(j->d, d_text, text_bytes, fill, d_out);
+    if (rc) return rc;
+    return job_rk(j, RK_MASK, mode, 0, d_text, d_offs, n, text_bytes, nullptr, nullptr, nullptr, nullptr, d_out, fill, stream);
 }
 
 int dach_job_wait(dach_job* j, uint64_t* needed) {
     if (!j) return DACH_INVALID_ARGUMENT;
+    if (j->unplaced) {  // the last placement's report would be stale
+        set_error("dach_job_wait: the job's scan has not been placed yet");
+        return DACH_INVALID_ARGUMENT;
+    }
+    if (j->rk != RK_MATCHES)  // a reduction: *needed = its total (0 for MASK, whose total stays at its zero)
+        return guarded([&]() -> int {
+            DeviceGuard g(j->d->device);
+            if (!g.ok) return DACH_CUDA_ERROR;
+            return finish_rk(nullptr, j->W, needed);
+        });
     if (!j->W.job_placed) {
         set_error("dach_job_wait: nothing has been placed yet");
         return DACH_INVALID_ARGUMENT;
@@ -3232,14 +3339,14 @@ double dach_job_scan_kernel_ms(const dach_job* j) {
     return 0;
 }
 
-// ms since the handle's first job scan of {scan kernel start, scan kernel end, peer push start, peer push end} of the job's
-// last step (the last two are 0 without a peer push): the timeline of a pipelined run
+// ms since the handle's first job operation of {scan kernel start, scan kernel end, peer push start, peer push end} of the
+// job's last step (the last two are 0 without a peer push, and after a reduction): the timeline of a pipelined run
 int dach_job_times(const dach_job* j, double out[4]) {
     if (!j || !out || !j->d->ev_ref) return DACH_INVALID_ARGUMENT;
     cudaEvent_t evs[4] = {j->W.ev[3], j->W.ev[1], j->W.ev_push[0], j->W.ev_push[1]};
     for (int i = 0; i < 4; ++i) {
         float ms = 0;
-        out[i] = cudaEventElapsedTime(&ms, j->d->ev_ref, evs[i]) == cudaSuccess ? ms : 0.0;
+        out[i] = (i < 2 || j->rk == RK_MATCHES) && cudaEventElapsedTime(&ms, j->d->ev_ref, evs[i]) == cudaSuccess ? ms : 0.0;
     }
     cudaGetLastError();
     return DACH_OK;
@@ -3247,7 +3354,7 @@ int dach_job_times(const dach_job* j, double out[4]) {
 
 double dach_job_push_ms(const dach_job* j) {
     float ms = 0;
-    if (j && cudaEventElapsedTime(&ms, j->W.ev_push[0], j->W.ev_push[1]) == cudaSuccess) return ms;
+    if (j && j->rk == RK_MATCHES && cudaEventElapsedTime(&ms, j->W.ev_push[0], j->W.ev_push[1]) == cudaSuccess) return ms;
     cudaGetLastError();
     return 0;
 }
@@ -3396,6 +3503,10 @@ int dach_group_place(dach_group* G, dach_job* j, uint64_t hay_base, int last, vo
         set_error("shard group: not connected");
         return DACH_INVALID_ARGUMENT;
     }
+    if (j->rk != RK_MATCHES) {
+        set_error("no scan to place: the job's last operation was a count, first-match, histogram or mask");
+        return DACH_INVALID_ARGUMENT;
+    }
     if (hay_base + j->W.job_n > G->n_total) {
         set_error("shard group: haystack range outside the gathered batch");
         return DACH_INVALID_ARGUMENT;
@@ -3439,6 +3550,7 @@ int dach_group_place(dach_group* G, dach_job* j, uint64_t hay_base, int last, vo
         const int rc = enqueue_place(j->d, W, G->out, G->match_cap, G->offs + hay_base, &G->ctl->base[step & 1], last != 0, st, nullptr,
                                      staged, dma, h_base, h_total);
         if (rc) return rc;
+        j->unplaced = false;
         k_group_signal_done<<<1, 1, 0, st>>>(G->peers.ctl[0], G->rank, step);
         ++j->d->launches;
         if (!cuda_ok(cudaGetLastError(), "shard group kernels")) return DACH_CUDA_ERROR;

@@ -236,8 +236,8 @@ int dach_dev_hist_stream(dach_dev *dev, int mode, int key, const uint8_t *d_text
  * The host forms copy text and offsets to the device in the slices of dach_scan_batch_host; only the
  * per-haystack results come back (8 B, or 13 B, per haystack; dach_dev_last_h2d_bytes / _d2h_bytes).
  * Option kernel = 1, 2 or 4 runs the default lane machines here (kernel = 3); kernel = 0 the lane-per-haystack
- * kernels.  Stream chunks have their own forms (dach_dev_count_stream, dach_dev_first_stream); jobs and shard
- * groups have no count / first form. */
+ * kernels.  Stream chunks have their own forms (dach_dev_count_stream, dach_dev_first_stream), jobs theirs
+ * (dach_job_count, dach_job_first); shard groups have no count / first form. */
 int dach_dev_count_batch(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
                          uint64_t text_bytes, uint64_t *d_counts, uint64_t *total, void *stream);
 int dach_count_batch_host(dach_dev *dev, int mode, const uint8_t *text, const uint64_t *offs, uint64_t n,
@@ -264,8 +264,8 @@ int dach_first_batch_host(dach_dev *dev, int mode, const uint8_t *text, const ui
  * The host form uses the slices of dach_scan_batch_host, adds them up on the device and copies
  * n_hist x 8 bytes back once (dach_dev_last_d2h_bytes).  Option hist_smem (default 1024; 0 = off):
  * events of the leading compact states are counted in shared memory per CTA first.  Options kernel and
- * the fallbacks as dach_dev_count_batch.  Stream chunks have dach_dev_hist_stream; jobs and shard groups have no
- * histogram form. */
+ * the fallbacks as dach_dev_count_batch.  Stream chunks have dach_dev_hist_stream, jobs dach_job_hist; shard groups
+ * have no histogram form. */
 typedef enum {
     DACH_KEY_OUTPUT = 0,
     DACH_KEY_VALUE = 1
@@ -297,7 +297,7 @@ int dach_hist_batch_host(dach_dev *dev, int mode, int key, const uint8_t *text, 
  * for both at the default, allocated at the handle's first DF call.  A window that would need more is scanned again as two halves (no DACH_OUTPUT_OVERFLOW);
  * dach_dev_last_df_windows reports the windows and re-scans of the handle's last DF call.
  * The device form copies the n + 1 offsets to the host once (8 B per haystack).  Jobs, stream chunks and
- * shard groups have no DF form. */
+ * shard groups have no DF form (each window needs a host round trip, and the pair sets belong to the handle). */
 int dach_dev_df_batch(dach_dev *dev, int mode, int key, const uint8_t *d_text, const uint64_t *d_offs,
                       uint64_t n, uint64_t text_bytes, uint64_t *d_df, uint64_t n_df, uint64_t *total,
                       void *stream);
@@ -319,8 +319,8 @@ int dach_dev_last_df_windows(const dach_dev *dev, uint64_t *windows, uint64_t *r
  * automaton and fill >= 0x80 (valid UTF-8 stays valid: spans start and end on char boundaries).  A span never
  * reaches before its haystack's first byte, whatever lengths a deserialized automaton carries.  The calls
  * synchronise `stream`.  The host form uses the slices of dach_scan_batch_host and copies each slice's masked
- * bytes back (dach_dev_last_d2h_bytes).  Options kernel and the fallbacks as dach_dev_count_batch; stream
- * chunks, jobs and shard groups have no mask form. */
+ * bytes back (dach_dev_last_d2h_bytes).  Options kernel and the fallbacks as dach_dev_count_batch.  Jobs have
+ * dach_job_mask; stream chunks and shard groups have no mask form. */
 int dach_dev_mask_batch(dach_dev *dev, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
                         uint64_t text_bytes, uint8_t fill, uint8_t *d_out, void *stream);
 int dach_mask_batch_host(dach_dev *dev, int mode, const uint8_t *text, const uint64_t *offs, uint64_t n,
@@ -339,10 +339,28 @@ int dach_mask_batch_host(dach_dev *dev, int mode, const uint8_t *text, const uin
  *                   d_base is a DEVICE pointer to the index of this batch's first match in d_out, or
  *                   NULL for 0; d_out / d_out_offs may be peer-mapped memory of another GPU.
  *   dach_job_wait   blocks until the placement is done; status and *needed as dach_dev_scan_batch.
+ *                   DACH_INVALID_ARGUMENT while a scan waits for its placement.
  * A job holds one scan at a time: scan -> place -> (wait) -> scan ...; the next dach_job_scan is
  * ordered after the previous placement by the library.  Options are read from the dach_dev.
  * A job keeps its dach_dev alive: dach_dev_free may come first (as a garbage collector may order
- * it); the device image is then released by the last dach_job_free of that device. */
+ * it); the device image is then released by the last dach_job_free of that device.
+ *
+ * Reductions on a job: count, first, hist and mask enqueue exactly what dach_dev_count_batch,
+ * dach_dev_first_batch, dach_dev_hist_batch and dach_dev_mask_batch run (same modes, keys, lane machines,
+ * segments, fallbacks and options; the results are theirs byte for byte) on `stream` and the job's own
+ * workspace, take no handle mutex and return at once.  Everything the synchronous call refuses before it
+ * runs is refused the same way here before anything is enqueued (null arguments, the mode, the histogram's
+ * key and size, an overlapping or non-ASCII charwise mask, more than 2^32 - 16 haystacks); so is a
+ * reduction while the job holds a scan that has not been placed.  hist ADDS into d_hist, and several jobs
+ * may add into one histogram at the same time.  A job still holds one operation at a time: each one is
+ * ordered after the job's previous one by the library, and scans and reductions may alternate on a job;
+ * dach_job_place after a reduction is DACH_INVALID_ARGUMENT (nothing to place).  Then dach_job_wait blocks
+ * until the work is done and sets *needed to the synchronous call's total (*total, *n_found; 0 for mask).
+ * Bad device offsets: dach_job_wait returns DACH_INVALID_ARGUMENT, and d_counts, d_first, d_found, d_hist
+ * and d_out are left as they were.  Jobs do not write the handle's dach_dev_last_* figures.  A job's
+ * histogram tables take 8 B per compact state plus 8 B per output record, allocated at its first hist.
+ * Document frequencies, stream chunks and shard groups have no job reduction (a DF window needs a host
+ * round trip, and its pair sets belong to the handle). */
 typedef struct dach_job dach_job;
 int dach_job_create(dach_dev *dev, dach_job **out);
 void dach_job_free(dach_job *job);
@@ -350,11 +368,20 @@ int dach_job_scan(dach_job *job, int mode, const uint8_t *d_text, const uint64_t
                   uint64_t text_bytes, uint64_t cap_matches, void *stream);
 int dach_job_place(dach_job *job, dach_match *d_out, uint64_t out_cap, uint64_t *d_out_offs,
                    const uint64_t *d_base, void *stream);
+int dach_job_count(dach_job *job, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                   uint64_t text_bytes, uint64_t *d_counts, void *stream);
+int dach_job_first(dach_job *job, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                   uint64_t text_bytes, dach_match *d_first, uint8_t *d_found, void *stream);
+int dach_job_hist(dach_job *job, int mode, int key, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                  uint64_t text_bytes, uint64_t *d_hist, uint64_t n_hist, void *stream);
+int dach_job_mask(dach_job *job, int mode, const uint8_t *d_text, const uint64_t *d_offs, uint64_t n,
+                  uint64_t text_bytes, uint8_t fill, uint8_t *d_out, void *stream);
 int dach_job_wait(dach_job *job, uint64_t *needed);
-double dach_job_scan_kernel_ms(const dach_job *job); /* CUDA-event time of the job's last scan kernel */
+double dach_job_scan_kernel_ms(const dach_job *job); /* CUDA-event time of the job's last scan kernel, any kind */
 double dach_job_push_ms(const dach_job *job);        /* ... of its last peer push (dach_group_place), 0 if none */
-/* ms since the handle's first dach_job_scan of {scan kernel start, scan kernel end, peer push start, peer push end}
- * of the job's last step: the timeline of a pipelined run (bench.py config.timeline) */
+/* ms since the handle's first job operation of {scan kernel start, scan kernel end, peer push start, peer push
+ * end} of the job's last step, whatever its kind (no push after a reduction: 0): the timeline of a pipelined run
+ * (bench.py config.timeline) */
 int dach_job_times(const dach_job *job, double out[4]);
 
 /* ---- shard groups: the exchange step of a batch sharded over the GPUs of one node ---------

@@ -131,6 +131,16 @@ extern "C" {
                          cap_matches: u64, stream: *mut c_void) -> i32;
     pub fn dach_job_place(job: *mut DachJob, d_out: *mut DachMatch, out_cap: u64, d_out_offs: *mut u64, d_base: *const u64,
                           stream: *mut c_void) -> i32;
+    /// Counts, first matches, histograms (ADDED into d_hist) and masked text on a job: the results of the
+    /// dach_dev_*_batch twins, only enqueued; dach_job_wait reports the twin's total (0 for the mask).
+    pub fn dach_job_count(job: *mut DachJob, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64, text_bytes: u64,
+                          d_counts: *mut u64, stream: *mut c_void) -> i32;
+    pub fn dach_job_first(job: *mut DachJob, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64, text_bytes: u64,
+                          d_first: *mut DachMatch, d_found: *mut u8, stream: *mut c_void) -> i32;
+    pub fn dach_job_hist(job: *mut DachJob, mode: i32, key: i32, d_text: *const u8, d_offs: *const u64, n: u64,
+                         text_bytes: u64, d_hist: *mut u64, n_hist: u64, stream: *mut c_void) -> i32;
+    pub fn dach_job_mask(job: *mut DachJob, mode: i32, d_text: *const u8, d_offs: *const u64, n: u64, text_bytes: u64,
+                         fill: u8, d_out: *mut u8, stream: *mut c_void) -> i32;
     pub fn dach_job_wait(job: *mut DachJob, needed: *mut u64) -> i32;
 
     /// Shard groups: every rank's placement stores its matches into rank 0's dense buffer over NVLink peer memory.

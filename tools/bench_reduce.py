@@ -719,6 +719,28 @@ def run_mask_output(args, W, pma, batches, dmode, omode, n, hay_len, step_bytes,
     }
 
 
+def device_batches(W, dev):
+    """The workload's batches on the device as bench.py makes them: [(text, offs)], and the bytes of text resident."""
+    import torch
+
+    from daachorse_b200 import synth as S
+
+    hay_len = W.hay_len
+    pool_t = torch.from_numpy(W.pool).to(dev)
+    starts_t = torch.from_numpy(W.starts).to(dev)
+    ranges = W.batch_ranges()
+    if "window" in W.spec:
+        text_all, offs_all = S.materialise_on_device(pool_t, starts_t, hay_len)
+        return [(text_all[lo * hay_len: hi * hay_len], offs_all[: hi - lo + 1]) for lo, hi in ranges], text_all.numel()
+    batches = []
+    for lo, hi in ranges:
+        t, o = S.materialise_on_device(pool_t, starts_t[lo:hi], hay_len)
+        if W.spec["synth"] == "C4":
+            S.pad_to_char_boundary_device(t, hi - lo, hay_len)
+        batches.append((t, o))
+    return batches, sum(b[0].numel() for b in batches)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--output", required=True, choices=["counts", "first", "hist", "df", "mask"])
@@ -746,8 +768,6 @@ def main():
 
     import torch
 
-    from daachorse_b200 import synth as S
-
     assert torch.cuda.is_available(), "bench_reduce.py needs a CUDA device (no CPU fallback)"
     torch.cuda.set_device(0)
     dev = torch.device("cuda", 0)
@@ -759,22 +779,7 @@ def main():
     for kv in args.option:
         k, v = kv.split("=")
         pma.set_option(k, int(v))
-    pool_t = torch.from_numpy(W.pool).to(dev)
-    starts_t = torch.from_numpy(W.starts).to(dev)
-    ranges = W.batch_ranges()
-    if "window" in W.spec:
-        text_all, offs_all = S.materialise_on_device(pool_t, starts_t, hay_len)
-        batches = [(text_all[lo * hay_len: hi * hay_len], offs_all[: hi - lo + 1]) for lo, hi in ranges]
-        resident = text_all.numel()
-    else:
-        batches = []
-        for lo, hi in ranges:
-            t, o = S.materialise_on_device(pool_t, starts_t[lo:hi], hay_len)
-            if W.spec["synth"] == "C4":
-                S.pad_to_char_boundary_device(t, hi - lo, hay_len)
-            batches.append((t, o))
-        resident = sum(b[0].numel() for b in batches)
-    del pool_t
+    batches, resident = device_batches(W, dev)
     n = W.window
     torch.cuda.synchronize()
     line = run_reduce_output(args, W, pma, batches, dmode, omode, n, hay_len, n * hay_len, resident, dev, t_setup)

@@ -8,7 +8,8 @@ native, so this is a subset of tests/test_gpu_parity.py that still launches ever
 Golden vectors (all iterators x bytewise / charwise), random batches on every kernel option, text buffers at odd
 addresses and with no slack after the last byte (the 8-byte text loads must not touch anything outside), stream
 chunks, event blocks with output lists of 255 and more (stored at the landing and through the event queue; k_expand in
-pool and output order), counts and first matches, per-pattern histograms (both keys, shared-memory counters on and off), document frequencies (both keys, the smallest pair table), asynchronous jobs, a two-rank shard group on one device.  Every result is checked against the oracle."""
+pool and output order), counts and first matches, per-pattern histograms (both keys, shared-memory counters on and off), document frequencies (both keys, the smallest pair table), asynchronous jobs (the matches and the four
+reductions), a two-rank shard group on one device.  Every result is checked against the oracle."""
 import json
 import os
 import sys
@@ -244,6 +245,44 @@ def masked_text():
                 n_scans += 1
 
 
+def job_reductions():
+    """dach_job_count / _first / _hist / _mask, one compact case each on two jobs and two streams (StdMachine3 in
+    segments and the lane-per-haystack loops); against the oracle."""
+    global n_scans
+    dev = torch.device("cuda", 0)
+    pma, opma, text, offs = random_case(90, False, 0)
+    mode = D.FIND_OVERLAPPING
+    ref = opma.scan_batch(ORC[mode], text, offs, want_matches=True)
+    counts = ref["counts"].astype(np.int64)
+    found = counts > 0
+    starts = np.concatenate([[0], np.cumsum(counts)])[:-1]
+    vals = pma.outputs()[0].astype(np.int64)
+    hist = np.bincount(ref["matches"]["value"].astype(np.int64), minlength=int(vals.max()) + 1)
+    mask = EM.expected_from_matches(text, offs, ref["matches"], ref["counts"], 0x2A)
+    t = torch.from_numpy(text.copy()).to(dev)
+    o = torch.from_numpy(offs.astype(np.int64)).to(dev)
+    jobs = [pma.job(0), pma.job(0)]
+    sts = [torch.cuda.Stream(dev), torch.cuda.Stream(dev)]
+    torch.cuda.synchronize()
+    for opts in ({"kernel": 3, "seg_len": 64}, {"kernel": 0}):
+        for k, v in opts.items():
+            pma.set_option(k, v)
+        for i, (job, st) in enumerate(zip(jobs, sts)):
+            c = job.count(mode, t, o, stream=st)
+            assert job.wait() == int(counts.sum()) and np.array_equal(c.cpu().numpy(), counts), opts
+            f, fd = job.first(mode, t, o, stream=st)
+            assert job.wait() == int(found.sum()) and np.array_equal(fd.cpu().numpy(), found), opts
+            assert f.cpu().numpy().astype(np.uint32)[found].tobytes() == ref["matches"][starts[found]].tobytes(), opts
+            h = job.pattern_counts(mode, t, o, key="value" if i == 0 else "output", stream=st)
+            assert job.wait() == len(ref["matches"]), opts
+            assert np.array_equal(h.cpu().numpy(), hist if i == 0 else hist[vals]), opts
+            m = job.mask(mode, t, o, fill=0x2A, stream=st)
+            assert job.wait() == 0 and np.array_equal(m.cpu().numpy(), mask), opts
+            n_scans += 4
+        pma.set_option("seg_len", 0)
+    pma.set_option("kernel", 3)
+
+
 def streams_jobs_groups():
     global n_scans
     dev = torch.device("cuda", 0)
@@ -318,6 +357,7 @@ if __name__ == "__main__":
     histograms()
     doc_frequencies()
     masked_text()
+    job_reductions()
     streams_jobs_groups()
     torch.cuda.synchronize()
     print("sanitize.py: %d scans, all equal to the oracle" % n_scans)
