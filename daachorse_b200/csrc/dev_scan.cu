@@ -32,6 +32,9 @@
 //                               counts published into every rank's control block, bases derived from them, done
 //                               flags -- system-scope releases, local polling; the packed matches go to rank 0 through
 //                               a copy engine (or k_push: destination-aligned 16-byte peer stores)
+// Host side: plan_scan (scan_plan.h, shared with the CPU emulators) picks the scan kernel and whether the batch is cut
+// into segments, launch_matches / launch_rk map its choice to one template instantiation and launch<K> launches it;
+// enqueue_rk takes its destinations as one RkOut; every host-buffer batch runs through the slices of run_slices.
 // No CPU fallback exists: every entry point here fails with DACH_CUDA_ERROR without a device.
 #include <cuda_runtime.h>
 
@@ -51,6 +54,7 @@
 #include "dev_image.h"
 #include "host.h"
 #include "scan_lane.cuh"
+#include "scan_plan.h"
 
 namespace dach {
 
@@ -1380,245 +1384,113 @@ struct DeviceGuard {
     }
 };
 
-template <bool CW, int MODE>
-cudaError_t launch_scan_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    static bool attr_done[kMaxDevices] = {};  // per instantiation and per device (the attribute is per device)
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(k_scan<CW, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
-    }
-    k_scan<CW, MODE><<<grid, threads, smem, st>>>(P);
-    return cudaGetLastError();
-}
+// One scan kernel's launch; the attribute is set once per kernel and per device (it is per device)
+struct Launch {
+    const ScanParams& P;
+    int grid, threads;
+    size_t smem;
+    cudaStream_t st;
+};
 
-template <class M, class LANE, int MAXT, int MINB, bool HOT>
-cudaError_t launch_machine_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    static bool attr_done[kMaxDevices] = {};  // per instantiation and per device
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(k_scan_machine<M, LANE, MAXT, MINB, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
-    }
-    k_scan_machine<M, LANE, MAXT, MINB, HOT><<<grid, threads, smem, st>>>(P);
-    return cudaGetLastError();
-}
-
-template <template <int> class M, class LANE, int MAXT, int MINB, bool HOT>
-cudaError_t launch_std_modes(int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    switch (mode) {
-        case M_FIND: return launch_machine_t<M<M_FIND>, LANE, MAXT, MINB, HOT>(P, grid, threads, smem, st);
-        case M_NO_SUFFIX: return launch_machine_t<M<M_NO_SUFFIX>, LANE, MAXT, MINB, HOT>(P, grid, threads, smem, st);
-        case M_OVERLAPPING: return launch_machine_t<M<M_OVERLAPPING>, LANE, MAXT, MINB, HOT>(P, grid, threads, smem, st);
-    }
-    return cudaErrorInvalidValue;
-}
-
-// bytewise Standard iterators: which = 3 StdMachine3 (hot records in shared memory if P.hot_entries), 2 StdMachine2,
-// 1 StdMachine; dense = two CTAs of up to 768 threads per SM (40 registers) instead of one of 1024
-cudaError_t launch_std(int which, int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st,
-                       bool dense) {
-    if (which >= 3) {
-        if (P.hot_entries)
-            return dense ? launch_std_modes<StdMachine3, Lane3, 768, 2, true>(mode, P, grid, threads, smem, st)
-                         : launch_std_modes<StdMachine3, Lane3, 1024, 1, true>(mode, P, grid, threads, smem, st);
-        return dense ? launch_std_modes<StdMachine3, Lane3, 768, 2, false>(mode, P, grid, threads, smem, st)
-                     : launch_std_modes<StdMachine3, Lane3, 1024, 1, false>(mode, P, grid, threads, smem, st);
-    }
-    if (which == 2)
-        return dense ? launch_std_modes<StdMachine2, Lane2, 768, 2, false>(mode, P, grid, threads, smem, st)
-                     : launch_std_modes<StdMachine2, Lane2, 1024, 1, false>(mode, P, grid, threads, smem, st);
-    return dense ? launch_std_modes<StdMachine, LaneStd, 768, 2, false>(mode, P, grid, threads, smem, st)
-                 : launch_std_modes<StdMachine, LaneStd, 1024, 1, false>(mode, P, grid, threads, smem, st);
-}
-
-template <int MODE, int MAXT, bool HOT>
-cudaError_t launch_duo_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
+// CARVEOUT (k_scan_direct): the smallest carveout that holds kDirectSmemBudget, so that L1 keeps what it has beside
+// the queue kernel
+template <auto K, bool CARVEOUT = false>
+cudaError_t launch(const Launch& L) {
     static bool attr_done[kMaxDevices] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(k_scan_duo<MODE, MAXT, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+        cudaError_t e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+        if (CARVEOUT && e == cudaSuccess) e = cudaFuncSetAttribute(K, cudaFuncAttributePreferredSharedMemoryCarveout, kDirectCarveoutPct);
         if (e != cudaSuccess) return e;
         if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
     }
-    k_scan_duo<MODE, MAXT, HOT><<<grid, threads, smem, st>>>(P);
+    K<<<L.grid, L.threads, L.smem, L.st>>>(L.P);
     return cudaGetLastError();
-}
-template <int MAXT, bool HOT>
-cudaError_t launch_duo_m(int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    switch (mode) {
-        case M_FIND: return launch_duo_t<M_FIND, MAXT, HOT>(P, grid, threads, smem, st);
-        case M_NO_SUFFIX: return launch_duo_t<M_NO_SUFFIX, MAXT, HOT>(P, grid, threads, smem, st);
-        case M_OVERLAPPING: return launch_duo_t<M_OVERLAPPING, MAXT, HOT>(P, grid, threads, smem, st);
-    }
-    return cudaErrorInvalidValue;
-}
-// two haystacks per lane (option kernel = 4): 1024 threads (64 registers) or up to 768 (85 registers)
-cudaError_t launch_duo(int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    if (threads > 768)
-        return P.hot_entries ? launch_duo_m<1024, true>(mode, P, grid, threads, smem, st) : launch_duo_m<1024, false>(mode, P, grid, threads, smem, st);
-    return P.hot_entries ? launch_duo_m<768, true>(mode, P, grid, threads, smem, st) : launch_duo_m<768, false>(mode, P, grid, threads, smem, st);
 }
 
-template <int MODE, bool HOT>
-cudaError_t launch_direct_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    static bool attr_done[kMaxDevices] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(k_scan_direct<MODE, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-        // the smallest carveout that holds kDirectSmemBudget: L1 keeps what it has beside the queue kernel
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(k_scan_direct<MODE, HOT>, cudaFuncAttributePreferredSharedMemoryCarveout, kDirectCarveoutPct);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
-    }
-    k_scan_direct<MODE, HOT><<<grid, threads, smem, st>>>(P);
-    return cudaGetLastError();
-}
-// StdMachine3's matches path without the queue (option event_queue = 0, one CTA per SM)
-cudaError_t launch_direct(int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
+// f(std::integral_constant<int, MODE>{}) for the run-time iterator `mode`
+template <class F>
+cudaError_t for_mode(int mode, F&& f) {
     switch (mode) {
-        case M_FIND:
-            return P.hot_entries ? launch_direct_t<M_FIND, true>(P, grid, threads, smem, st) : launch_direct_t<M_FIND, false>(P, grid, threads, smem, st);
-        case M_NO_SUFFIX:
-            return P.hot_entries ? launch_direct_t<M_NO_SUFFIX, true>(P, grid, threads, smem, st)
-                                 : launch_direct_t<M_NO_SUFFIX, false>(P, grid, threads, smem, st);
-        case M_OVERLAPPING:
-            return P.hot_entries ? launch_direct_t<M_OVERLAPPING, true>(P, grid, threads, smem, st)
-                                 : launch_direct_t<M_OVERLAPPING, false>(P, grid, threads, smem, st);
+        case M_FIND: return f(std::integral_constant<int, M_FIND>{});
+        case M_OVERLAPPING: return f(std::integral_constant<int, M_OVERLAPPING>{});
+        case M_NO_SUFFIX: return f(std::integral_constant<int, M_NO_SUFFIX>{});
+        case M_LEFTMOST: return f(std::integral_constant<int, M_LEFTMOST>{});
     }
     return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_cw(int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    switch (mode) {
-        case M_FIND: return launch_machine_t<CwMachine<M_FIND>, LaneCw, 1024, 1, false>(P, grid, threads, smem, st);
-        case M_OVERLAPPING: return launch_machine_t<CwMachine<M_OVERLAPPING>, LaneCw, 1024, 1, false>(P, grid, threads, smem, st);
-        case M_NO_SUFFIX: return launch_machine_t<CwMachine<M_NO_SUFFIX>, LaneCw, 1024, 1, false>(P, grid, threads, smem, st);
-        default: return launch_machine_t<CwMachine<M_LEFTMOST>, LaneCw, 1024, 1, false>(P, grid, threads, smem, st);
+// bytewise Standard lane machines: dense = two CTAs of up to 768 threads per SM (40 registers) instead of one of 1024
+template <class M, class LANE, bool HOT>
+cudaError_t launch_std(const Launch& L, bool dense) {
+    return dense ? launch<k_scan_machine<M, LANE, 768, 2, HOT>>(L) : launch<k_scan_machine<M, LANE, 1024, 1, HOT>>(L);
+}
+
+// The matches scan of iterator MODE on machine m.  HOT: StdMachine3 stages P.hot_entries records in shared memory.
+template <int MODE>
+cudaError_t launch_matches(Machine m, bool cw, const Launch& L, bool dense) {
+    const bool hot = L.P.hot_entries != 0;
+    if constexpr (MODE == M_LEFTMOST) {
+        if (m == Machine::Lm) return launch<k_scan_machine<LmMachine, LaneLm, 1024, 1, false>>(L);
+    } else {
+        switch (m) {
+            case Machine::Std: return launch_std<StdMachine<MODE>, LaneStd, false>(L, dense);
+            case Machine::Std2: return launch_std<StdMachine2<MODE>, Lane2, false>(L, dense);
+            case Machine::Std3: return hot ? launch_std<StdMachine3<MODE>, Lane3, true>(L, dense) : launch_std<StdMachine3<MODE>, Lane3, false>(L, dense);
+            case Machine::Std3Direct: return hot ? launch<k_scan_direct<MODE, true>, true>(L) : launch<k_scan_direct<MODE, false>, true>(L);
+            case Machine::Duo:  // 1024 threads (64 registers) or up to 768 (85 registers)
+                if (L.threads > 768) return hot ? launch<k_scan_duo<MODE, 1024, true>>(L) : launch<k_scan_duo<MODE, 1024, false>>(L);
+                return hot ? launch<k_scan_duo<MODE, 768, true>>(L) : launch<k_scan_duo<MODE, 768, false>>(L);
+            default: break;
+        }
     }
+    if (m == Machine::Cw) return launch<k_scan_machine<CwMachine<MODE>, LaneCw, 1024, 1, false>>(L);
+    return cw ? launch<k_scan<true, MODE>>(L) : launch<k_scan<false, MODE>>(L);
 }
 
-cudaError_t launch_lm(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    return launch_machine_t<LmMachine, LaneLm, 1024, 1, false>(P, grid, threads, smem, st);
-}
-
-cudaError_t launch_scan(bool cw, int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    switch ((cw ? 4 : 0) + mode) {
-        case 0: return launch_scan_t<false, M_FIND>(P, grid, threads, smem, st);
-        case 1: return launch_scan_t<false, M_OVERLAPPING>(P, grid, threads, smem, st);
-        case 2: return launch_scan_t<false, M_NO_SUFFIX>(P, grid, threads, smem, st);
-        case 3: return launch_scan_t<false, M_LEFTMOST>(P, grid, threads, smem, st);
-        case 4: return launch_scan_t<true, M_FIND>(P, grid, threads, smem, st);
-        case 5: return launch_scan_t<true, M_OVERLAPPING>(P, grid, threads, smem, st);
-        case 6: return launch_scan_t<true, M_NO_SUFFIX>(P, grid, threads, smem, st);
-        case 7: return launch_scan_t<true, M_LEFTMOST>(P, grid, threads, smem, st);
+// The scan of result kind RK (COUNT, FIRST, FIRST_STREAM, HIST, DF, MASK) of iterator MODE on machine m.  FIRST is
+// built for M_OVERLAPPING and M_LEFTMOST only (plan_scan folds the Standard iterators), FIRST_STREAM for the stream
+// steppers find / find_overlapping on StdMachine3 and CwMachine only (plan_scan refuses the others).
+template <int RK, int MODE>
+cudaError_t launch_rk(Machine m, bool cw, const Launch& L) {
+    constexpr bool built = RK == RK_FIRST ? MODE == M_OVERLAPPING || MODE == M_LEFTMOST
+                           : RK == RK_FIRST_STREAM ? MODE == M_FIND || MODE == M_OVERLAPPING
+                                                   : true;
+    if constexpr (built) {
+        if constexpr (MODE != M_LEFTMOST)
+            if (m == Machine::Std3)
+                return L.P.hot_entries ? launch<k_scan_machine_rk<StdMachine3<MODE>, Lane3, MODE, RK, true>>(L)
+                                       : launch<k_scan_machine_rk<StdMachine3<MODE>, Lane3, MODE, RK, false>>(L);
+        if (m == Machine::Cw) return launch<k_scan_machine_rk<CwMachine<MODE>, LaneCw, MODE, RK, false>>(L);
+        if constexpr (RK != RK_FIRST_STREAM) {
+            if constexpr (MODE == M_LEFTMOST)
+                if (m == Machine::Lm) return launch<k_scan_machine_rk<LmMachine, LaneLm, M_LEFTMOST, RK, false>>(L);
+            if (m == Machine::Lane) return cw ? launch<k_scan_rk<true, MODE, RK>>(L) : launch<k_scan_rk<false, MODE, RK>>(L);
+        }
     }
     return cudaErrorInvalidValue;
 }
 
-// ---- COUNT / FIRST launchers: StdMachine3, LmMachine, CwMachine, or the lane-per-haystack kernels --------------
-template <class M, class LANE, int MODE, int RK, bool HOT>
-cudaError_t launch_rk_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    static bool attr_done[kMaxDevices] = {};  // per instantiation and per device
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(k_scan_machine_rk<M, LANE, MODE, RK, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
-    }
-    k_scan_machine_rk<M, LANE, MODE, RK, HOT><<<grid, threads, smem, st>>>(P);
-    return cudaGetLastError();
-}
-template <bool CW, int MODE, int RK>
-cudaError_t launch_scan_rk_t(const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    static bool attr_done[kMaxDevices] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= kMaxDevices || !attr_done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(k_scan_rk<CW, MODE, RK>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < kMaxDevices) attr_done[dev] = true;
-    }
-    k_scan_rk<CW, MODE, RK><<<grid, threads, smem, st>>>(P);
-    return cudaGetLastError();
-}
-
-// which: 3 StdMachine3 (bytewise Standard), 1 LmMachine / CwMachine (by the automaton), 0 lane per haystack.
-// FIRST only runs M_OVERLAPPING (Standard) and M_LEFTMOST: the caller folds the Standard modes.  HIST and DF run all
-// of COUNT's kernels.
 template <int RK>
-cudaError_t launch_rk(int which, bool cw, int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    if (which == 3) {
-        switch (mode) {
-            case M_FIND:
-                if constexpr (RK != RK_FIRST)
-                    return P.hot_entries ? launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, RK, true>(P, grid, threads, smem, st)
-                                         : launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, RK, false>(P, grid, threads, smem, st);
-                break;
-            case M_NO_SUFFIX:
-                if constexpr (RK != RK_FIRST)
-                    return P.hot_entries ? launch_rk_t<StdMachine3<M_NO_SUFFIX>, Lane3, M_NO_SUFFIX, RK, true>(P, grid, threads, smem, st)
-                                         : launch_rk_t<StdMachine3<M_NO_SUFFIX>, Lane3, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
-                break;
-            case M_OVERLAPPING:
-                return P.hot_entries ? launch_rk_t<StdMachine3<M_OVERLAPPING>, Lane3, M_OVERLAPPING, RK, true>(P, grid, threads, smem, st)
-                                     : launch_rk_t<StdMachine3<M_OVERLAPPING>, Lane3, M_OVERLAPPING, RK, false>(P, grid, threads, smem, st);
-        }
-        return cudaErrorInvalidValue;
-    }
-    if (which == 1 && cw) {
-        switch (mode) {
-            case M_FIND:
-                if constexpr (RK != RK_FIRST) return launch_rk_t<CwMachine<M_FIND>, LaneCw, M_FIND, RK, false>(P, grid, threads, smem, st);
-                break;
-            case M_NO_SUFFIX:
-                if constexpr (RK != RK_FIRST) return launch_rk_t<CwMachine<M_NO_SUFFIX>, LaneCw, M_NO_SUFFIX, RK, false>(P, grid, threads, smem, st);
-                break;
-            case M_OVERLAPPING: return launch_rk_t<CwMachine<M_OVERLAPPING>, LaneCw, M_OVERLAPPING, RK, false>(P, grid, threads, smem, st);
-            case M_LEFTMOST: return launch_rk_t<CwMachine<M_LEFTMOST>, LaneCw, M_LEFTMOST, RK, false>(P, grid, threads, smem, st);
-        }
-        return cudaErrorInvalidValue;
-    }
-    if (which == 1) return mode == M_LEFTMOST ? launch_rk_t<LmMachine, LaneLm, M_LEFTMOST, RK, false>(P, grid, threads, smem, st) : cudaErrorInvalidValue;
-    switch ((cw ? 4 : 0) + mode) {
-        case 0: if constexpr (RK != RK_FIRST) return launch_scan_rk_t<false, M_FIND, RK>(P, grid, threads, smem, st); break;
-        case 1: return launch_scan_rk_t<false, M_OVERLAPPING, RK>(P, grid, threads, smem, st);
-        case 2: if constexpr (RK != RK_FIRST) return launch_scan_rk_t<false, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
-        case 3: return launch_scan_rk_t<false, M_LEFTMOST, RK>(P, grid, threads, smem, st);
-        case 4: if constexpr (RK != RK_FIRST) return launch_scan_rk_t<true, M_FIND, RK>(P, grid, threads, smem, st); break;
-        case 5: return launch_scan_rk_t<true, M_OVERLAPPING, RK>(P, grid, threads, smem, st);
-        case 6: if constexpr (RK != RK_FIRST) return launch_scan_rk_t<true, M_NO_SUFFIX, RK>(P, grid, threads, smem, st); break;
-        case 7: return launch_scan_rk_t<true, M_LEFTMOST, RK>(P, grid, threads, smem, st);
-    }
-    return cudaErrorInvalidValue;
+cudaError_t launch_rk_modes(int mode, Machine m, bool cw, const Launch& L) {
+    return for_mode(mode, [&](auto M) { return launch_rk<RK, decltype(M)::value>(m, cw, L); });
 }
 
-// FIRST of stream chunks: the caller's iterator (find / find_overlapping) on StdMachine3 or CwMachine
-cudaError_t launch_first_stream(bool cw, int mode, const ScanParams& P, int grid, int threads, size_t smem, cudaStream_t st) {
-    constexpr int R = RK_FIRST_STREAM;
-    if (cw)
-        return mode == M_FIND ? launch_rk_t<CwMachine<M_FIND>, LaneCw, M_FIND, R, false>(P, grid, threads, smem, st)
-                              : launch_rk_t<CwMachine<M_OVERLAPPING>, LaneCw, M_OVERLAPPING, R, false>(P, grid, threads, smem, st);
-    if (mode == M_FIND)
-        return P.hot_entries ? launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, R, true>(P, grid, threads, smem, st)
-                             : launch_rk_t<StdMachine3<M_FIND>, Lane3, M_FIND, R, false>(P, grid, threads, smem, st);
-    return P.hot_entries ? launch_rk_t<StdMachine3<M_OVERLAPPING>, Lane3, M_OVERLAPPING, R, true>(P, grid, threads, smem, st)
-                         : launch_rk_t<StdMachine3<M_OVERLAPPING>, Lane3, M_OVERLAPPING, R, false>(P, grid, threads, smem, st);
+// DACH_INVALID_ARGUMENT, with its reason for dach_last_error
+int invalid(const char* why) {
+    set_error(why);
+    return DACH_INVALID_ARGUMENT;
+}
+
+int check_stream_mode(int mode) {
+    if (mode != DACH_FIND && mode != DACH_FIND_OVERLAPPING)
+        return invalid("stream chunks: mode must be DACH_FIND or DACH_FIND_OVERLAPPING (the crate's two steppers)");
+    return DACH_OK;
 }
 
 int check_mode(const dach_dev* d, int mode) {
-    if (mode < DACH_FIND || mode > DACH_LEFTMOST_FIND) {
-        set_error("unknown scan mode");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (mode < DACH_FIND || mode > DACH_LEFTMOST_FIND) return invalid("unknown scan mode");
     const bool lm = is_leftmost(d->match_kind);
     if ((mode == DACH_LEFTMOST_FIND) != lm) {
         set_error(lm ? "Error: match_kind must be standard." : "Error: match_kind must be leftmost.");
@@ -1695,6 +1567,33 @@ size_t plan_smem(const dach_dev* d, ScanParams& P, bool v1, bool std3, int threa
     return smem;
 }
 
+// The scan kernel's persistent grid: CTAs = SMs (less option reserve_sms) x ctas_per_sm
+struct LaunchShape {
+    int threads, ctas_per_sm, grid;
+};
+LaunchShape launch_shape(const dach_dev* d) {
+    LaunchShape S;
+    S.threads = (int)std::min<int64_t>(std::max<int64_t>(d->opt_threads, 32), kMaxThreads) / 32 * 32;
+    S.ctas_per_sm = (int)std::min<int64_t>(std::max<int64_t>(d->opt_ctas_per_sm, 1), 2048 / S.threads);
+    const int free_sms = (int)std::min<int64_t>(std::max<int64_t>(d->opt_reserve_sms, 0), d->sm_count - 1);
+    S.grid = (d->sm_count - free_sms) * S.ctas_per_sm;
+    return S;
+}
+
+// plan_scan for this automaton and the handle's options
+ScanPlan plan_of(const dach_dev* d, int rk, int mode, bool stream, const LaunchShape& S) {
+    return plan_scan({.opt_kernel = d->opt_kernel, .compact = d->d_crec != nullptr, .charwise = d->charwise, .root_opos = d->root_opos != 0,
+                      .root_base = d->root_base != 0, .segmentable = d->segmentable, .opt_seg_len = d->opt_seg_len,
+                      .ctas_per_sm = S.ctas_per_sm, .opt_event_queue = d->opt_event_queue, .stream = stream,
+                      .matches = rk == RK_MATCHES, .first = rk == RK_FIRST, .mode = mode});
+}
+
+int refuse_stream() {
+    set_error("stream chunks need a Standard lane machine (find / find_overlapping, at most 2^24 states, bytewise: "
+              "BASE(ROOT) != 0, no empty pattern for find)");
+    return DACH_INVALID_ARGUMENT;
+}
+
 // segment table: counts per haystack -> first item per haystack (W.seg_first) -> (haystack, begin) per item
 void enqueue_seg_table(dach_dev* d, Workspace& W, const uint64_t* d_offs, uint64_t n, uint32_t seg_len, uint32_t seg_from,
                        ScanParams& P, cudaStream_t st) {
@@ -1725,10 +1624,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
                  uint64_t text_bytes, const uint64_t* d_offs, uint64_t n, uint64_t cap_matches, cudaStream_t st,
                  uint32_t* d_state_io = nullptr) {
     W.refused = false;
-    if (n > 0xfffffff0ull) {
-        set_error("too many haystacks in one batch (max 2^32-16)");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (n > 0xfffffff0ull) return invalid("too many haystacks in one batch (max 2^32-16)");
     // the previous placement out of this workspace (possibly on another stream) must be done before its
     // buffers are rewritten
     if (W.job_open) cudaStreamWaitEvent(st, W.ev_placed, 0);
@@ -1751,66 +1647,29 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
         cudaEventRecord(W.ev_scanned, st);
         return DACH_OK;
     }
-    int threads = (int)std::min<int64_t>(std::max<int64_t>(d->opt_threads, 32), kMaxThreads);
-    threads = (threads / 32) * 32;
-    int ctas_per_sm = (int)std::min<int64_t>(std::max<int64_t>(d->opt_ctas_per_sm, 1), 2048 / threads);
-    const int free_sms = (int)std::min<int64_t>(std::max<int64_t>(d->opt_reserve_sms, 0), d->sm_count - 1);
-    const int grid = (d->sm_count - free_sms) * ctas_per_sm;
-    // the lane machines serve every iterator of both automata except find_iter with an empty pattern
-    // (it only reports zero-length matches, src/bytewise/iter.rs:60-85), which keeps the simple kernel
-    const bool v1 = d->opt_kernel >= 1 && d->d_crec && !(mode == M_FIND && d->root_opos != 0);
-    const bool cw_machine = v1 && d->charwise;
-    const bool lm_machine = v1 && !d->charwise && mode == M_LEFTMOST;
-    // StdMachine2 / StdMachine3 keep ROOT's record in registers and probe it like any state: needs BASE(ROOT) != 0
-    const bool std2 = v1 && !d->charwise && mode != M_LEFTMOST && d->opt_kernel >= 2 && d->root_base != 0;
-    const bool std3 = std2 && d->opt_kernel >= 3;
-    const bool duo = std3 && d->opt_kernel >= 4 && ctas_per_sm == 1;
-    const bool events = std3 && !duo;  // StdMachine3's matches path stores events (k_scan_machine / k_scan_direct)
-    // ... at their landing, without the queue: one CTA per SM, whose shared memory the staged records fill
-    const bool direct = events && ctas_per_sm == 1 && d->opt_event_queue == 0;
-
-    if (d_state_io && !std2 && !cw_machine) {
-        set_error("stream chunks need a Standard lane machine (find / find_overlapping, at most 2^24 states, bytewise: "
-                  "BASE(ROOT) != 0, no empty pattern for find)");
-        return DACH_INVALID_ARGUMENT;
-    }
-
-    // Work items.  find_overlapping / no_suffix may cut haystacks into segments (exact with an
-    // (L-1)-byte warm-up, SURVEY.md Appendix C.1) so that small batches and long haystacks still
-    // fill the machine; everything else works on whole haystacks.
-    // (a chunk of a stream resumes in a given state: it stays one item)
-    bool seg = v1 && !d->charwise && !d_state_io && (mode == M_OVERLAPPING || mode == M_NO_SUFFIX) && d->opt_seg_len >= 0 && d->segmentable;
+    const LaunchShape S = launch_shape(d);
+    const ScanPlan plan = plan_of(d, RK_MATCHES, mode, d_state_io != nullptr, S);
+    if (plan.refused) return refuse_stream();
+    const bool events = plan.events();
+    bool seg = plan.seg;
     uint32_t seg_len = 0, seg_from = 0;
     uint64_t n_items_max = n;
     if (seg) {
-        const uint64_t lanes = (uint64_t)grid * threads;
+        const uint64_t lanes = (uint64_t)S.grid * S.threads;
         const uint64_t warm = d->max_pattern_len ? d->max_pattern_len - 1 : 0;
-        const uint64_t floor_len = std::max<uint64_t>(256, 8 * warm);  // warm-up overhead <= 1/8
-        uint64_t want;
-        uint64_t tail_bytes = text_bytes;
-        if (d->opt_seg_len > 0) {
-            want = (uint64_t)d->opt_seg_len;
-        } else if (d->opt_tail_seg && n >= 4 * lanes && n < 0xffffffffull) {
+        if (d->opt_seg_len <= 0 && d->opt_tail_seg && n >= 4 * lanes && n < 0xffffffffull) {
             // plenty of haystacks per lane: only the tail of the batch is cut, so that lanes that finish
             // early find short items instead of idling through the last wave
             const uint64_t n_tail = 2 * lanes;
             seg_from = (uint32_t)(n - n_tail);
-            want = std::max(text_bytes / n / 8 + 1, floor_len);
             // the item tables are sized from the exact byte count of the tail (two 8-byte reads)
             cudaMemcpyAsync(&W.pinned->tail_offs[0], d_offs + seg_from, 8, cudaMemcpyDeviceToHost, st);
             cudaMemcpyAsync(&W.pinned->tail_offs[1], d_offs + n, 8, cudaMemcpyDeviceToHost, st);
             if (!cuda_ok(cudaStreamSynchronize(st), "read tail size")) return DACH_CUDA_ERROR;
-            tail_bytes = W.pinned->tail_offs[1] - W.pinned->tail_offs[0];
+            seg = seg_cut(std::max(text_bytes / n / 8 + 1, seg_floor(warm)), text_bytes, W.pinned->tail_offs[1] - W.pinned->tail_offs[0], n,
+                          &seg_len, &n_items_max);
         } else {
-            want = std::max(text_bytes / (2 * lanes) + 1, floor_len);  // ~2 items per lane
-        }
-        want = (want + 255) & ~uint64_t(255);
-        if (want >= text_bytes || want >= (1ull << 31)) {
-            seg = false;  // every haystack fits one segment
-        } else {
-            seg_len = (uint32_t)want;
-            n_items_max = n + tail_bytes / seg_len + 1;
-            if (n_items_max > 0xfffffff0ull) seg = false, n_items_max = n;
+            seg = seg_cut(seg_want(d->opt_seg_len, text_bytes, lanes, warm), text_bytes, text_bytes, n, &seg_len, &n_items_max);
         }
     }
     const uint64_t n_tiles = (n_items_max + kScanTile - 1) / kScanTile;
@@ -1831,7 +1690,8 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
     P.pool_blocks = pool_blocks;
     P.ctrl = static_cast<ScanCtrl*>(W.ctrl.p);
     P.state_io = d_state_io;
-    const size_t smem = plan_smem(d, P, v1, std3, threads, ctas_per_sm, duo ? 2 : direct ? 0 : 1);
+    const int queue_sets = plan.machine == Machine::Duo ? 2 : plan.machine == Machine::Std3Direct ? 0 : 1;
+    const size_t smem = plan_smem(d, P, plan.lane_machine(), plan.std3(), S.threads, S.ctas_per_sm, queue_sets);
 
     unsigned long long* tiles = static_cast<unsigned long long*>(W.tiles.p);
     unsigned long long* item_offs = static_cast<unsigned long long*>(W.item_offs.p);
@@ -1843,13 +1703,9 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
         enqueue_seg_table(d, W, d_offs, n, seg_len, seg_from, P, st);
     }
     cudaEventRecord(W.ev[3], st);
-    if (!cuda_ok(cw_machine   ? launch_cw(mode, P, grid, std::min(threads, 1024), smem, st)
-                 : lm_machine ? launch_lm(P, grid, std::min(threads, 1024), smem, st)
-                 : duo        ? launch_duo(mode, P, grid, threads, smem, st)
-                 : direct     ? launch_direct(mode, P, grid, threads, smem, st)
-                 : v1        ? launch_std(std3 ? 3 : std2 ? 2 : 1, mode, P, grid, threads, smem, st,
-                                           ctas_per_sm >= 2 && threads <= 768 && grid % 2 == 0)
-                              : launch_scan(d->charwise, mode, P, grid, threads, smem, st),
+    const bool dense = S.ctas_per_sm >= 2 && S.threads <= 768 && S.grid % 2 == 0;
+    const Launch L{P, S.grid, S.threads, smem, st};
+    if (!cuda_ok(for_mode(plan.mode, [&](auto M) { return launch_matches<decltype(M)::value>(plan.machine, d->charwise, L, dense); }),
                  "k_scan launch"))
         return DACH_CUDA_ERROR;
     cudaEventRecord(W.ev[1], st);
@@ -1901,10 +1757,7 @@ int enqueue_scan(dach_dev* d, Workspace& W, int mode, const uint8_t* d_text, con
 int enqueue_place(dach_dev* d, Workspace& W, dach_match* d_out, uint64_t out_cap, uint64_t* d_out_offs,
                   const unsigned long long* d_base, bool last, cudaStream_t st, const uint32_t* d_pos_in = nullptr,
                   bool staged = false, bool dma = false, uint64_t h_base = 0, uint64_t h_total = 0) {
-    if (!W.job_open) {
-        set_error("no scan to place");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!W.job_open) return invalid("no scan to place");
     if (st != W.job_stream) cudaStreamWaitEvent(st, W.ev_scanned, 0);
     const uint64_t n = W.job_n, n_items = W.job_items;
     const ScanCtrl* ctrl = static_cast<const ScanCtrl*>(W.ctrl.p);
@@ -1991,10 +1844,9 @@ int finish_scan(dach_dev* d, Workspace& W, uint64_t out_cap, uint64_t* needed) {
     // every carry of a per-item u32 count is 2^32 matches item_offs[n] does not hold (count_carry, scan_lane.cuh)
     const uint64_t total = W.pinned->total + ((uint64_t)W.pinned->ctrl.carries << 32);
     if (needed) *needed = total;
-    if (W.pinned->ctrl.bad_offsets) {
-        set_error("haystack offsets must be ascending and inside text_bytes, and no haystack may reach 4 GiB (match positions are u32)");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (W.pinned->ctrl.bad_offsets)
+        return invalid("haystack offsets must be ascending and inside text_bytes, "
+                       "and no haystack may reach 4 GiB (match positions are u32)");
     if (W.pinned->ctrl.carries) {
         // no capacity helps: the match list of one haystack is indexed in 32 bits
         W.refused = true;
@@ -2030,14 +1882,8 @@ double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::
 
 int check_host_offsets(const uint64_t* offs, uint64_t n) {
     for (uint64_t i = 0; i < n; ++i) {
-        if (offs[i + 1] < offs[i]) {
-            set_error("haystack offsets must be ascending");
-            return DACH_INVALID_ARGUMENT;
-        }
-        if (offs[i + 1] - offs[i] > 0xffffffffull) {
-            set_error("a haystack is longer than 4 GiB - 1 (match positions are u32)");
-            return DACH_INVALID_ARGUMENT;
-        }
+        if (offs[i + 1] < offs[i]) return invalid("haystack offsets must be ascending");
+        if (offs[i + 1] - offs[i] > 0xffffffffull) return invalid("a haystack is longer than 4 GiB - 1 (match positions are u32)");
     }
     return DACH_OK;
 }
@@ -2129,12 +1975,72 @@ bool slice_h2d(dach_dev* d, Workspace& W, const uint8_t* text, const uint64_t* o
     return true;
 }
 
+// A slice on its slot: W's text and offsets hold haystacks [s.first, s.last) of the caller's batch
+struct SliceOnSlot {
+    Workspace& W;
+    Slice& s;
+    uint64_t tb, ns;         // its text bytes and haystacks
+    const uint8_t* d_text;   // d_text + offs[i] addresses haystack i in W.text
+    const uint8_t* lo() const { return static_cast<const uint8_t*>(W.text.p); }
+    const uint8_t* end() const { return lo() + tb; }
+    const uint64_t* d_offs() const { return static_cast<const uint64_t*>(W.offs.p); }
+};
+
+struct SliceRun {
+    std::vector<Slice> slices;
+    double t_reuse = 0, t_final = 0;  // waiting for slot reuse, for the final synchronisation (ms)
+};
+
+// Runs a host-buffer batch (n > 0) through the slots: the offsets are checked, the batch is cut into slices for
+// iterator `mode`, the slots are made ready, then prepare() runs, and body(k, slice) for every slice k on its slot
+// while the uploads of the next two slices are queued.  Every slot's stream is synchronised before this returns, on
+// every exit: whatever is queued there reads the caller's text or writes the caller's buffers.
+template <class Prepare, class Body>
+int run_slices(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, const char* sync_what, SliceRun& run,
+               Prepare&& prepare, Body&& body) {
+    int rc = check_host_offsets(offs, n);
+    if (rc) return rc;
+    struct Drain {
+        dach_dev* d;
+        ~Drain() {
+            for (Workspace& w : d->slot)
+                if (w.stream) cudaStreamSynchronize(w.stream);
+        }
+    } drain_on_exit{d};
+    std::vector<Slice>& slices = run.slices;
+    slices = cut_slices(d, mode, offs, n);
+    for (Workspace& w : d->slot)
+        if (!w.init(true)) return DACH_CUDA_ERROR;
+    rc = prepare();
+    if (rc) return rc;
+    auto issue_h2d = [&](size_t k) -> bool {
+        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &run.t_reuse);
+    };
+    // The copy engine must never wait for the host: the host blocks in body() until slice k is scanned, so the
+    // uploads of the next TWO slices are queued before that (with one slice ahead the H2D engine idles for the length
+    // of every scan).
+    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
+    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
+    for (size_t k = 0; k < slices.size(); ++k) {
+        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
+        Workspace& W = d->slot[k % dach_dev::kSlots];
+        Slice& s = slices[k];
+        const uint64_t tb = offs[s.last] - offs[s.first];
+        rc = body(k, SliceOnSlot{W, s, tb, s.last - s.first, static_cast<const uint8_t*>(W.text.p) - offs[s.first]});
+        if (rc) return rc;
+    }
+    const double t_f0 = now_ms();
+    for (Workspace& w : d->slot)
+        if (!cuda_ok(cudaStreamSynchronize(w.stream), sync_what)) return DACH_CUDA_ERROR;
+    run.t_final = now_ms() - t_f0;
+    return DACH_OK;
+}
+
+int no_prepare() { return DACH_OK; }
+
 int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n,
                          dach_match* out, uint64_t out_cap, uint64_t* out_offs, uint64_t* needed) {
-    if (!d || !offs || !out_offs || (out_cap && !out)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!d || !offs || !out_offs || (out_cap && !out)) return invalid("null argument");
     int rc = check_mode(d, mode);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(d->mu);
@@ -2146,82 +2052,59 @@ int scan_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
         if (needed) *needed = 0;
         return DACH_OK;
     }
-    rc = check_host_offsets(offs, n);
-    if (rc) return rc;
-    // whatever is still queued on the slots' streams reads the caller's text or writes the caller's buffers:
-    // no exit from here on may leave it in flight
-    struct Drain {
-        dach_dev* d;
-        ~Drain() {
-            for (Workspace& w : d->slot)
-                if (w.stream) cudaStreamSynchronize(w.stream);
-        }
-    } drain_on_exit{d};
-    std::vector<Slice> slices = cut_slices(d, mode, offs, n);
-    for (Workspace& w : d->slot)
-        if (!w.init(true)) return DACH_CUDA_ERROR;
-    // every slot's previous work must be finished before its buffers are reused
     bool overflow = false, refused = false;
     uint64_t base = 0;
     const bool trace = getenv("DACH_DEBUG") != nullptr;
-    double t_reuse = 0, t_scan = 0, t_final = 0, gpu_ms = 0;
-    auto now = now_ms;
-    const double t_begin = now();
-    auto issue_h2d = [&](size_t k) -> bool {
-        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
+    double t_scan = 0, gpu_ms = 0, t_begin = 0;
+    auto start_clock = [&]() {  // the trace's total runs from the slots being ready, as the slices are issued
+        t_begin = now_ms();
+        return DACH_OK;
     };
-    // The copy engine must never wait for the host: the host blocks in scan_locked() until slice k is
-    // scanned, so the uploads of the next TWO slices are queued before that (with one slice ahead the
-    // H2D engine idles for the length of every scan).
-    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
-    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
-    for (size_t k = 0; k < slices.size(); ++k) {
-        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
-        Workspace& W = d->slot[k % dach_dev::kSlots];
-        Slice& s = slices[k];
-        const uint64_t tb = offs[s.last] - offs[s.first], ns = s.last - s.first;
+    SliceRun run;
+    rc = run_slices(d, mode, text, offs, n, "D2H", run, start_clock, [&](size_t k, const SliceOnSlot& x) -> int {
+        Workspace& W = x.W;
+        Slice& s = x.s;
         s.base = base;
         // device-side capacity of this slice: what is left of the caller's buffer, bounded by a
         // generous per-slice estimate that grows if a slice overflows it
-        uint64_t cap = std::max<uint64_t>(std::max<uint64_t>(tb / 4, 4096), W.out.bytes > 16 ? (W.out.bytes - 16) / 12 : 0);
-        const double t_s0 = now();
+        uint64_t cap = std::max<uint64_t>(std::max<uint64_t>(x.tb / 4, 4096), W.out.bytes > 16 ? (W.out.bytes - 16) / 12 : 0);
+        const double t_s0 = now_ms();
+        int r;
         for (;;) {
             if (!ensure(W.out, cap * 12 + 16)) return DACH_CUDA_ERROR;
             uint64_t total = 0;
-            const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
-            rc = scan_locked(d, W, mode, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb, tb, static_cast<const uint64_t*>(W.offs.p), ns,
-                             static_cast<dach_match*>(W.out.p), cap, static_cast<uint64_t*>(W.out_offs.p), &total, W.stream);
+            r = scan_locked(d, W, mode, x.d_text, x.lo(), x.end(), x.tb, x.d_offs(), x.ns, static_cast<dach_match*>(W.out.p), cap,
+                            static_cast<uint64_t*>(W.out_offs.p), &total, W.stream);
             s.total = total;
-            if (rc == DACH_OUTPUT_OVERFLOW && total > cap) {
+            if (r == DACH_OUTPUT_OVERFLOW && total > cap) {
                 cap = total;
                 continue;
             }
             break;
         }
-        t_scan += now() - t_s0;
+        t_scan += now_ms() - t_s0;
         gpu_ms += d->last_total_ms;
         // a haystack past 2^32 matches: nothing is copied back, the other slices are still counted for *needed
-        if (rc == DACH_INVALID_ARGUMENT && W.refused) refused = true;
-        else if (rc != DACH_OK && rc != DACH_OUTPUT_OVERFLOW) return rc;
+        if (r == DACH_INVALID_ARGUMENT && W.refused) refused = true;
+        else if (r != DACH_OK && r != DACH_OUTPUT_OVERFLOW) return r;
         if (refused || base + s.total > out_cap) overflow = true;
         if (!overflow) {
             // the slice's final offset is the next slice's first one: only the last slice copies it
-            const uint64_t no = (k + 1 == slices.size()) ? ns + 1 : ns;
+            const uint64_t no = (k + 1 == run.slices.size()) ? x.ns + 1 : x.ns;
             if (!cuda_ok(cudaMemcpyAsync(out_offs + s.first, W.out_offs.p, no * 8, cudaMemcpyDeviceToHost, W.stream), "D2H offsets"))
                 return DACH_CUDA_ERROR;
             if (s.total && !cuda_ok(cudaMemcpyAsync(out + base, W.out.p, s.total * 12, cudaMemcpyDeviceToHost, W.stream), "D2H matches"))
                 return DACH_CUDA_ERROR;
-            d->last_d2h += (ns + 1) * 8 + s.total * 12;
+            d->last_d2h += (x.ns + 1) * 8 + s.total * 12;
         }
         base += s.total;
-    }
-    const double t_f0 = now();
-    for (Workspace& w : d->slot)
-        if (!cuda_ok(cudaStreamSynchronize(w.stream), "D2H")) return DACH_CUDA_ERROR;
-    t_final = now() - t_f0;
+        return DACH_OK;
+    });
+    if (rc) return rc;
+    const std::vector<Slice>& slices = run.slices;
     if (trace)
         fprintf(stderr, "dach_scan_batch_host: %zu slices, %.2f ms total: waiting for slot reuse %.2f, in scan_locked %.2f, final D2H wait %.2f; kernels %.2f ms\n",
-                slices.size(), now() - t_begin, t_reuse, t_scan, t_final, gpu_ms);
+                slices.size(), now_ms() - t_begin, run.t_reuse, t_scan, run.t_final, gpu_ms);
     if (needed) *needed = base;
     if (refused) {
         char buf[256];
@@ -2255,24 +2138,30 @@ DfSet df_set(dach_dev* d, int i) {
 }
 
 // ---- COUNT / FIRST / HIST / DF: the scan of a batch and its results on one stream.  No synchronisation. -----------
-// rk = RK_COUNT: d_counts (n x u64); RK_FIRST: d_first (n tuples), d_found (n x u8); RK_HIST: added into d_hist by
-// `key` (DACH_KEY_OUTPUT / DACH_KEY_VALUE; the caller has checked its size); RK_DF: one window (df_windows), added
-// into d_hist by `key` unless W.pinned->ctrl.overflow is set once W.ev_placed has completed.  The total (matches, or haystacks with a
-// match) lands in W.pinned->total_rk once W.ev_placed has completed.  No block pool, no offsets, no gather: options
-// kernel = 1, 2, 4 run StdMachine3 here (kernel = 0: the lane-per-haystack kernels).
-// d_state_io (stream chunks, dach_dev_*_stream): haystack i is the next chunk of stream i, resumed in and leaving its
-// state there as in enqueue_scan; FIRST then runs the caller's iterator to each chunk's last byte (RK_FIRST_STREAM)
-// and adds d_pos (or nothing) to its positions.  Stream chunks are never cut into segments.
-// rk = RK_MASK: d_masked (in the text's coordinates, like d_text) receives [text_lo, text_end) of the text, then `fill`
-// over every match; no post-pass.
+// Where enqueue_rk's results go (device memory).  RK_COUNT: counts (n x u64); RK_FIRST: first (n tuples), found (n x
+// u8); RK_HIST: added into hist by `key` (DACH_KEY_OUTPUT / DACH_KEY_VALUE; the caller has checked its size); RK_DF: one
+// window (df_windows), added into hist by `key` unless W.pinned->ctrl.overflow is set once W.ev_placed has completed;
+// RK_MASK: masked (in the text's coordinates, like d_text) receives [text_lo, text_end) of the text, then `fill` over
+// every match.  state (stream chunks, dach_dev_*_stream): haystack i is the next chunk of stream i, resumed in and
+// leaving its state there as in enqueue_scan; FIRST then runs the caller's iterator to each chunk's last byte
+// (RK_FIRST_STREAM) and adds pos (or nothing) to its positions.
+struct RkOut {
+    uint64_t* counts = nullptr;
+    dach_match* first = nullptr;
+    uint8_t* found = nullptr;
+    int key = 0;
+    uint64_t* hist = nullptr;
+    uint32_t* state = nullptr;
+    const uint32_t* pos = nullptr;
+    uint8_t* masked = nullptr;
+    uint8_t fill = 0;
+};
+
+// The total (matches, or haystacks with a match) lands in W.pinned->total_rk once W.ev_placed has completed.  No block
+// pool, no offsets, no gather.  Stream chunks are never cut into segments; MASK has no post-pass.
 int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_text, const uint8_t* text_lo, const uint8_t* text_end,
-               uint64_t text_bytes, const uint64_t* d_offs, uint64_t n, uint64_t* d_counts, dach_match* d_first, uint8_t* d_found,
-               cudaStream_t st, int key = 0, uint64_t* d_hist = nullptr, uint32_t* d_state_io = nullptr, const uint32_t* d_pos = nullptr,
-               uint8_t* d_masked = nullptr, uint8_t fill = 0) {
-    if (n > 0xfffffff0ull) {
-        set_error("too many haystacks in one batch (max 2^32-16)");
-        return DACH_INVALID_ARGUMENT;
-    }
+               uint64_t text_bytes, const uint64_t* d_offs, uint64_t n, const RkOut& o, cudaStream_t st) {
+    if (n > 0xfffffff0ull) return invalid("too many haystacks in one batch (max 2^32-16)");
     if (W.job_open) cudaStreamWaitEvent(st, W.ev_placed, 0);
     if (!ensure(W.ctrl, sizeof(ScanCtrl)) || !ensure(W.total_rk, 8)) return DACH_CUDA_ERROR;
     if (!cuda_ok(cudaMemsetAsync(W.ctrl.p, 0, sizeof(ScanCtrl), st), "memset ctrl") ||
@@ -2286,45 +2175,20 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         const uint64_t bytes = (uint64_t)(text_end - text_lo);
         if (rk != RK_MASK || bytes == 0) return;
         const uint64_t blocks = std::min<uint64_t>((bytes / 16 + 256) / 256, 16ull * d->sm_count);
-        k_mask_copy<<<(unsigned)blocks, 256, 0, st>>>(text_lo, d_masked + (text_lo - d_text), bytes, static_cast<const ScanCtrl*>(W.ctrl.p));
+        k_mask_copy<<<(unsigned)blocks, 256, 0, st>>>(text_lo, o.masked + (text_lo - d_text), bytes, static_cast<const ScanCtrl*>(W.ctrl.p));
         ++d->launches;
     };
     if (n > 0) {
-        int threads = (int)std::min<int64_t>(std::max<int64_t>(d->opt_threads, 32), kMaxThreads);
-        threads = (threads / 32) * 32;
-        const int ctas_per_sm = (int)std::min<int64_t>(std::max<int64_t>(d->opt_ctas_per_sm, 1), 2048 / threads);
-        const int free_sms = (int)std::min<int64_t>(std::max<int64_t>(d->opt_reserve_sms, 0), d->sm_count - 1);
-        const int grid = (d->sm_count - free_sms) * ctas_per_sm;
-        // the first event of a haystack is the same for all three Standard iterators: FIRST runs find_overlapping
-        // (not on a stream: the state carried after a find match is not the find_overlapping one)
-        const int mmode = (rk == RK_FIRST && mode != M_LEFTMOST && !d_state_io) ? M_OVERLAPPING : mode;
-        const bool v1 = d->opt_kernel >= 1 && d->d_crec && !(mmode == M_FIND && d->root_opos != 0);
-        const bool cw_machine = v1 && d->charwise;
-        const bool lm_machine = v1 && !d->charwise && mmode == M_LEFTMOST;
-        const bool std3 = v1 && !d->charwise && mmode != M_LEFTMOST && d->root_base != 0;
-        const bool machine = cw_machine || lm_machine || std3;
-        if (d_state_io && !std3 && !cw_machine) {  // as enqueue_scan
-            set_error("stream chunks need a Standard lane machine (find / find_overlapping, at most 2^24 states, bytewise: "
-                      "BASE(ROOT) != 0, no empty pattern for find)");
-            return DACH_INVALID_ARGUMENT;
-        }
-        // segments as in enqueue_scan (no tail-only cutting; a chunk of a stream resumes in a given state: it stays one item)
-        bool seg = std3 && !d_state_io && (mmode == M_OVERLAPPING || mmode == M_NO_SUFFIX) && d->opt_seg_len >= 0 && d->segmentable;
+        const LaunchShape S = launch_shape(d);
+        const ScanPlan plan = plan_of(d, rk, mode, o.state != nullptr, S);
+        if (plan.refused) return refuse_stream();
+        const bool machine = plan.lane_machine();
+        // no tail-only cutting here
         uint32_t seg_len = 0;
         uint64_t n_items_max = n;
-        if (seg) {
-            const uint64_t lanes = (uint64_t)grid * threads;
-            const uint64_t warm = d->max_pattern_len ? d->max_pattern_len - 1 : 0;
-            uint64_t want = d->opt_seg_len > 0 ? (uint64_t)d->opt_seg_len : std::max(text_bytes / (2 * lanes) + 1, std::max<uint64_t>(256, 8 * warm));
-            want = (want + 255) & ~uint64_t(255);
-            if (want >= text_bytes || want >= (1ull << 31)) {
-                seg = false;
-            } else {
-                seg_len = (uint32_t)want;
-                n_items_max = n + text_bytes / seg_len + 1;
-                if (n_items_max > 0xfffffff0ull) seg = false, n_items_max = n;
-            }
-        }
+        const bool seg = plan.seg && seg_cut(seg_want(d->opt_seg_len, text_bytes, (uint64_t)S.grid * S.threads,
+                                                      d->max_pattern_len ? d->max_pattern_len - 1 : 0),
+                                             text_bytes, text_bytes, n, &seg_len, &n_items_max);
         const uint64_t n_tiles = (n + kScanTile - 1) / kScanTile;
         if ((rk == RK_COUNT || rk == RK_FIRST) && !ensure(W.items_rk, n_items_max * (rk == RK_FIRST ? 16 : 8))) return DACH_CUDA_ERROR;
         if (seg && (!ensure(W.tiles, n_tiles * 8) || !ensure(W.nseg, n * 4) || !ensure(W.seg_first, (n + 1) * 8) ||
@@ -2334,7 +2198,7 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
         P.ctrl = static_cast<ScanCtrl*>(W.ctrl.p);
         P.item_count = static_cast<unsigned long long*>(W.items_rk.p);
         P.item_first = static_cast<uint4*>(W.items_rk.p);
-        P.state_io = d_state_io;
+        P.state_io = o.state;
         uint32_t hist_k = 0;
         if (rk == RK_HIST) {
             if (machine) hist_k = (uint32_t)std::min<int64_t>(std::max<int64_t>(d->opt_hist_smem, 0), std::min<int64_t>(d->n_cslots, 16384));
@@ -2348,26 +2212,27 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
             P.hist_smem = hist_k;
         }
         if (rk == RK_DF) {  // the sets are empty here (df_prepare, then k_df_clear after every window)
-            P.df_key_value = key == DACH_KEY_VALUE;
+            P.df_key_value = o.key == DACH_KEY_VALUE;
             P.df_slots = df_set(d, 0);
             P.df_keys = df_set(d, 1);
         }
-        P.mask_out = d_masked;
-        P.mask_fill = fill;
-        const size_t smem = plan_smem(d, P, machine, std3, threads, ctas_per_sm, 1, hist_k);
+        P.mask_out = o.masked;
+        P.mask_fill = o.fill;
+        const size_t smem = plan_smem(d, P, machine, plan.std3(), S.threads, S.ctas_per_sm, 1, hist_k);
         k_check_offsets<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_offs, n, (uint64_t)(text_end - d_text), P.ctrl);
         ++d->launches;
         mask_copy();
         if (seg) enqueue_seg_table(d, W, d_offs, n, seg_len, 0, P, st);
         cudaEventRecord(W.ev[3], st);
-        const int which = std3 ? 3 : machine ? 1 : 0;
-        const int t = machine ? std::min(threads, 1024) : threads;
-        if (!cuda_ok(rk == RK_COUNT  ? launch_rk<RK_COUNT>(which, d->charwise, mmode, P, grid, t, smem, st)
-                     : rk == RK_HIST ? launch_rk<RK_HIST>(which, d->charwise, mmode, P, grid, t, smem, st)
-                     : rk == RK_DF   ? launch_rk<RK_DF>(which, d->charwise, mmode, P, grid, t, smem, st)
-                     : rk == RK_MASK ? launch_rk<RK_MASK>(which, d->charwise, mmode, P, grid, t, smem, st)
-                     : d_state_io    ? launch_first_stream(d->charwise, mmode, P, grid, t, smem, st)
-                                     : launch_rk<RK_FIRST>(which, d->charwise, mmode, P, grid, t, smem, st),
+        const Launch L{P, S.grid, S.threads, smem, st};
+        const Machine m = plan.machine;
+        const bool cw = d->charwise;
+        if (!cuda_ok(rk == RK_COUNT  ? launch_rk_modes<RK_COUNT>(plan.mode, m, cw, L)
+                     : rk == RK_HIST ? launch_rk_modes<RK_HIST>(plan.mode, m, cw, L)
+                     : rk == RK_DF   ? launch_rk_modes<RK_DF>(plan.mode, m, cw, L)
+                     : rk == RK_MASK ? launch_rk_modes<RK_MASK>(plan.mode, m, cw, L)
+                     : o.state       ? launch_rk_modes<RK_FIRST_STREAM>(plan.mode, m, cw, L)
+                                     : launch_rk_modes<RK_FIRST>(plan.mode, m, cw, L),
                      "k_scan launch"))
             return DACH_CUDA_ERROR;
         cudaEventRecord(W.ev[1], st);
@@ -2380,31 +2245,31 @@ int enqueue_rk(dach_dev* d, Workspace& W, int rk, int mode, const uint8_t* d_tex
                 ++d->launches;
             }
             const unsigned fb = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((d->n_outputs + 255) / 256, 8 * d->sm_count));
-            unsigned long long* hist = reinterpret_cast<unsigned long long*>(d_hist);
-            if (machine && mmode == M_OVERLAPPING)
-                k_hist_fold<true><<<fb, 256, 0, st>>>(P.rec_hist, d->d_outputs, d->n_outputs, key, hist, total);
+            unsigned long long* hist = reinterpret_cast<unsigned long long*>(o.hist);
+            if (machine && plan.mode == M_OVERLAPPING)
+                k_hist_fold<true><<<fb, 256, 0, st>>>(P.rec_hist, d->d_outputs, d->n_outputs, o.key, hist, total);
             else
-                k_hist_fold<false><<<fb, 256, 0, st>>>(P.rec_hist, d->d_outputs, d->n_outputs, key, hist, total);
+                k_hist_fold<false><<<fb, 256, 0, st>>>(P.rec_hist, d->d_outputs, d->n_outputs, o.key, hist, total);
             ++d->launches;
         } else if (rk == RK_DF) {
             // lane machines: (haystack, slot) -> (haystack, key); then the window's pairs into d_hist (the call's
             // accumulator) unless it overflowed, and both sets emptied for the next window
             const unsigned fb = (unsigned)(8 * d->sm_count);
-            if (machine && mmode == M_OVERLAPPING)
+            if (machine && plan.mode == M_OVERLAPPING)
                 k_df_expand<true><<<fb, 256, 0, st>>>(P);
             else if (machine)
                 k_df_expand<false><<<fb, 256, 0, st>>>(P);
-            k_df_add<<<fb, 256, 0, st>>>(P.df_keys, P.ctrl, reinterpret_cast<unsigned long long*>(d_hist), total);
+            k_df_add<<<fb, 256, 0, st>>>(P.df_keys, P.ctrl, reinterpret_cast<unsigned long long*>(o.hist), total);
             k_df_clear<<<fb, 256, 0, st>>>(P.df_slots, P.df_keys);
             d->launches += machine ? 3 : 2;
             if (!cuda_ok(cudaMemsetAsync(d->df_n.p, 0, 8, st), "memset pair counts")) return DACH_CUDA_ERROR;
         } else if (rk == RK_COUNT)
-            k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(d_counts), total, P.ctrl);
+            k_count_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_count, n, reinterpret_cast<unsigned long long*>(o.counts), total, P.ctrl);
         else if (rk == RK_MASK) {
-        } else if (d_state_io)
-            k_first_stream<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(P.item_first, n, d_pos, reinterpret_cast<uint32_t*>(d_first), d_found, total, P.ctrl);
+        } else if (o.state)
+            k_first_stream<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(P.item_first, n, o.pos, reinterpret_cast<uint32_t*>(o.first), o.found, total, P.ctrl);
         else
-            k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(d_first), d_found, total, P.ctrl);
+            k_first_hay<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg_first, P.item_first, n, reinterpret_cast<uint32_t*>(o.first), o.found, total, P.ctrl);
         if (rk == RK_COUNT || rk == RK_FIRST) d->launches += 2;  // the scan and k_count_hay / k_first_hay
         else ++d->launches;                                    // the scan
         if (!cuda_ok(cudaGetLastError(), "kernel launch")) return DACH_CUDA_ERROR;
@@ -2428,10 +2293,9 @@ int finish_rk(dach_dev* d, Workspace& W, uint64_t* total) {
     float ms = 0;
     if (d && cudaEventElapsedTime(&ms, W.ev[3], W.ev[1]) == cudaSuccess) d->last_scan_ms = ms;
     if (d && cudaEventElapsedTime(&ms, W.ev[0], W.ev[2]) == cudaSuccess) d->last_total_ms = ms;
-    if (W.pinned->ctrl.bad_offsets) {
-        set_error("haystack offsets must be ascending and inside text_bytes, and no haystack may reach 4 GiB (match positions are u32)");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (W.pinned->ctrl.bad_offsets)
+        return invalid("haystack offsets must be ascending and inside text_bytes, "
+                       "and no haystack may reach 4 GiB (match positions are u32)");
     if (total) *total = W.pinned->total_rk;
     return DACH_OK;
 }
@@ -2439,10 +2303,7 @@ int finish_rk(dach_dev* d, Workspace& W, uint64_t* total) {
 // COUNT / FIRST of a host-buffer batch: the slices of dach_scan_batch_host; only the per-haystack results come back
 int rk_batch_host_impl(dach_dev* d, int rk, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* counts,
                        dach_match* first, uint8_t* found, uint64_t* total) {
-    if (!d || !offs || (n && (rk == RK_COUNT ? !counts : (!first || !found)))) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!d || !offs || (n && (rk == RK_COUNT ? !counts : (!first || !found)))) return invalid("null argument");
     int rc = check_mode(d, mode);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(d->mu);
@@ -2451,53 +2312,34 @@ int rk_batch_host_impl(dach_dev* d, int rk, int mode, const uint8_t* text, const
     d->last_h2d = d->last_d2h = 0;
     if (total) *total = 0;
     if (n == 0) return DACH_OK;
-    rc = check_host_offsets(offs, n);
-    if (rc) return rc;
-    struct Drain {  // no exit may leave copies of the caller's buffers in flight
-        dach_dev* d;
-        ~Drain() {
-            for (Workspace& w : d->slot)
-                if (w.stream) cudaStreamSynchronize(w.stream);
-        }
-    } drain_on_exit{d};
-    const std::vector<Slice> slices = cut_slices(d, (rk == RK_FIRST && mode != M_LEFTMOST) ? M_OVERLAPPING : mode, offs, n);
-    for (Workspace& w : d->slot)
-        if (!w.init(true)) return DACH_CUDA_ERROR;
-    double t_reuse = 0;
-    auto issue_h2d = [&](size_t k) -> bool {
-        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
-    };
-    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
-    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
     uint64_t sum = 0;
-    for (size_t k = 0; k < slices.size(); ++k) {
-        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
-        Workspace& W = d->slot[k % dach_dev::kSlots];
-        const Slice& s = slices[k];
-        const uint64_t tb = offs[s.last] - offs[s.first], ns = s.last - s.first;
-        if (!ensure(W.out, ns * sizeof(dach_match) + 16)) return DACH_CUDA_ERROR;
-        const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
+    SliceRun run;
+    rc = run_slices(d, (rk == RK_FIRST && mode != M_LEFTMOST) ? M_OVERLAPPING : mode, text, offs, n, "D2H", run, no_prepare,
+                    [&](size_t, const SliceOnSlot& x) -> int {
+        Workspace& W = x.W;
+        const Slice& s = x.s;
+        if (!ensure(W.out, x.ns * sizeof(dach_match) + 16)) return DACH_CUDA_ERROR;
         // COUNT: counts in W.out; FIRST: tuples in W.out, found flags in W.out_offs
-        rc = enqueue_rk(d, W, rk, mode, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb, tb,
-                        static_cast<const uint64_t*>(W.offs.p), ns, static_cast<uint64_t*>(W.out.p), static_cast<dach_match*>(W.out.p),
-                        static_cast<uint8_t*>(W.out_offs.p), W.stream);
+        const RkOut o{.counts = static_cast<uint64_t*>(W.out.p), .first = static_cast<dach_match*>(W.out.p),
+                      .found = static_cast<uint8_t*>(W.out_offs.p)};
+        int r = enqueue_rk(d, W, rk, mode, x.d_text, x.lo(), x.end(), x.tb, x.d_offs(), x.ns, o, W.stream);
         uint64_t t = 0;
-        if (!rc) rc = finish_rk(d, W, &t);
-        if (rc) return rc;
+        if (!r) r = finish_rk(d, W, &t);
+        if (r) return r;
         sum += t;
         if (rk == RK_COUNT) {
-            if (!cuda_ok(cudaMemcpyAsync(counts + s.first, W.out.p, ns * 8, cudaMemcpyDeviceToHost, W.stream), "D2H counts"))
+            if (!cuda_ok(cudaMemcpyAsync(counts + s.first, W.out.p, x.ns * 8, cudaMemcpyDeviceToHost, W.stream), "D2H counts"))
                 return DACH_CUDA_ERROR;
-            d->last_d2h += ns * 8;
+            d->last_d2h += x.ns * 8;
         } else {
-            if (!cuda_ok(cudaMemcpyAsync(first + s.first, W.out.p, ns * sizeof(dach_match), cudaMemcpyDeviceToHost, W.stream), "D2H first") ||
-                !cuda_ok(cudaMemcpyAsync(found + s.first, W.out_offs.p, ns, cudaMemcpyDeviceToHost, W.stream), "D2H found"))
+            if (!cuda_ok(cudaMemcpyAsync(first + s.first, W.out.p, x.ns * sizeof(dach_match), cudaMemcpyDeviceToHost, W.stream), "D2H first") ||
+                !cuda_ok(cudaMemcpyAsync(found + s.first, W.out_offs.p, x.ns, cudaMemcpyDeviceToHost, W.stream), "D2H found"))
                 return DACH_CUDA_ERROR;
-            d->last_d2h += ns * (sizeof(dach_match) + 1);
+            d->last_d2h += x.ns * (sizeof(dach_match) + 1);
         }
-    }
-    for (Workspace& w : d->slot)
-        if (!cuda_ok(cudaStreamSynchronize(w.stream), "D2H")) return DACH_CUDA_ERROR;
+        return DACH_OK;
+    });
+    if (rc) return rc;
     if (total) *total = sum;
     return DACH_OK;
 }
@@ -2505,23 +2347,16 @@ int rk_batch_host_impl(dach_dev* d, int rk, int mode, const uint8_t* text, const
 // MASK: the fill byte of a charwise automaton keeps UTF-8 valid, and the masked buffer does not overlap the text (a lane
 // that has not read its bytes yet would see another lane's fill: spans reach back into the segment before theirs)
 int check_mask(const dach_dev* d, const uint8_t* text, uint64_t text_bytes, uint8_t fill, const uint8_t* out) {
-    if (d->charwise && fill >= 0x80) {
-        set_error("the fill byte of a charwise automaton must be below 0x80 (the masked text stays valid UTF-8)");
-        return DACH_INVALID_ARGUMENT;
-    }
-    if (text_bytes && (uintptr_t)out < (uintptr_t)text + text_bytes && (uintptr_t)text < (uintptr_t)out + text_bytes) {
-        set_error("the masked buffer overlaps the text (masking in place is not supported)");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (d->charwise && fill >= 0x80)
+        return invalid("the fill byte of a charwise automaton must be below 0x80 (the masked text stays valid UTF-8)");
+    if (text_bytes && (uintptr_t)out < (uintptr_t)text + text_bytes && (uintptr_t)text < (uintptr_t)out + text_bytes)
+        return invalid("the masked buffer overlaps the text (masking in place is not supported)");
     return DACH_OK;
 }
 
 // MASK of a host-buffer batch: the slices of dach_scan_batch_host; each slice's masked bytes come back into out
 int mask_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, uint8_t fill, uint8_t* out) {
-    if (!d || !offs || (offs[n] && (!text || !out))) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!d || !offs || (offs[n] && (!text || !out))) return invalid("null argument");
     int rc = check_mask(d, text, offs[n], fill, out);
     if (rc) return rc;
     rc = check_mode(d, mode);
@@ -2534,52 +2369,29 @@ int mask_batch_host_impl(dach_dev* d, int mode, const uint8_t* text, const uint6
         if (offs[0]) memcpy(out, text, offs[0]);
         return DACH_OK;
     }
-    rc = check_host_offsets(offs, n);
-    if (rc) return rc;
-    struct Drain {  // no exit may leave copies of the caller's buffers in flight
-        dach_dev* d;
-        ~Drain() {
-            for (Workspace& w : d->slot)
-                if (w.stream) cudaStreamSynchronize(w.stream);
-        }
-    } drain_on_exit{d};
-    const std::vector<Slice> slices = cut_slices(d, mode, offs, n);
-    for (Workspace& w : d->slot)
-        if (!w.init(true)) return DACH_CUDA_ERROR;
-    if (offs[0]) memcpy(out, text, offs[0]);  // bytes before the first haystack
-    double t_reuse = 0;
-    auto issue_h2d = [&](size_t k) -> bool {
-        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
+    SliceRun run;
+    auto copy_head = [&]() {
+        if (offs[0]) memcpy(out, text, offs[0]);  // bytes before the first haystack
+        return DACH_OK;
     };
-    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
-    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
-    for (size_t k = 0; k < slices.size(); ++k) {
-        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
-        Workspace& W = d->slot[k % dach_dev::kSlots];
-        const Slice& s = slices[k];
-        const uint64_t tb = offs[s.last] - offs[s.first], ns = s.last - s.first;
-        if (!ensure(W.out, tb + 16)) return DACH_CUDA_ERROR;
-        const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
-        rc = enqueue_rk(d, W, RK_MASK, mode, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb, tb,
-                        static_cast<const uint64_t*>(W.offs.p), ns, nullptr, nullptr, nullptr, W.stream, 0, nullptr, nullptr, nullptr,
-                        static_cast<uint8_t*>(W.out.p) - offs[s.first], fill);
-        if (!rc) rc = finish_rk(d, W, nullptr);
-        if (rc) return rc;
-        if (tb && !cuda_ok(cudaMemcpyAsync(out + offs[s.first], W.out.p, tb, cudaMemcpyDeviceToHost, W.stream), "D2H masked text"))
+    return run_slices(d, mode, text, offs, n, "D2H", run, copy_head, [&](size_t, const SliceOnSlot& x) -> int {
+        Workspace& W = x.W;
+        const Slice& s = x.s;
+        if (!ensure(W.out, x.tb + 16)) return DACH_CUDA_ERROR;
+        const RkOut o{.masked = static_cast<uint8_t*>(W.out.p) - offs[s.first], .fill = fill};
+        int r = enqueue_rk(d, W, RK_MASK, mode, x.d_text, x.lo(), x.end(), x.tb, x.d_offs(), x.ns, o, W.stream);
+        if (!r) r = finish_rk(d, W, nullptr);
+        if (r) return r;
+        if (x.tb && !cuda_ok(cudaMemcpyAsync(out + offs[s.first], W.out.p, x.tb, cudaMemcpyDeviceToHost, W.stream), "D2H masked text"))
             return DACH_CUDA_ERROR;
-        d->last_d2h += tb;
-    }
-    for (Workspace& w : d->slot)
-        if (!cuda_ok(cudaStreamSynchronize(w.stream), "D2H")) return DACH_CUDA_ERROR;
-    return DACH_OK;
+        d->last_d2h += x.tb;
+        return DACH_OK;
+    });
 }
 
 // HIST: the key and the size of the caller's histogram, decided before anything is launched
 int check_hist(const dach_dev* d, int key, uint64_t n_hist) {
-    if (key != DACH_KEY_OUTPUT && key != DACH_KEY_VALUE) {
-        set_error("unknown histogram key");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (key != DACH_KEY_OUTPUT && key != DACH_KEY_VALUE) return invalid("unknown histogram key");
     if (key == DACH_KEY_OUTPUT ? n_hist < d->n_outputs : (d->n_outputs && n_hist <= d->max_value)) {
         set_error(key == DACH_KEY_OUTPUT ? "n_hist is below the number of output records"
                                          : "n_hist must exceed the largest pattern value");
@@ -2592,10 +2404,7 @@ int check_hist(const dach_dev* d, int key, uint64_t n_hist) {
 // and is added into the caller's
 int hist_batch_host_impl(dach_dev* d, int mode, int key, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* hist,
                          uint64_t n_hist, uint64_t* total) {
-    if (!d || !offs || (n_hist && !hist)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!d || !offs || (n_hist && !hist)) return invalid("null argument");
     int rc = check_hist(d, key, n_hist);
     if (rc) return rc;
     rc = check_mode(d, mode);
@@ -2606,45 +2415,26 @@ int hist_batch_host_impl(dach_dev* d, int mode, int key, const uint8_t* text, co
     d->last_h2d = d->last_d2h = 0;
     if (total) *total = 0;
     if (n == 0) return DACH_OK;
-    rc = check_host_offsets(offs, n);
-    if (rc) return rc;
-    struct Drain {  // no exit may leave copies of the caller's buffers in flight
-        dach_dev* d;
-        ~Drain() {
-            for (Workspace& w : d->slot)
-                if (w.stream) cudaStreamSynchronize(w.stream);
-        }
-    } drain_on_exit{d};
-    const std::vector<Slice> slices = cut_slices(d, mode, offs, n);
-    for (Workspace& w : d->slot)
-        if (!w.init(true)) return DACH_CUDA_ERROR;
-    // the batch's histogram: zeroed before any slice adds into it (the slices run on the slots' streams)
     DevBuf& acc = d->slot[0].hist_acc;
-    if (!ensure(acc, n_hist * 8) || !cuda_ok(cudaMemsetAsync(acc.p, 0, n_hist * 8, d->slot[0].stream), "memset histogram") ||
-        !cuda_ok(cudaStreamSynchronize(d->slot[0].stream), "memset histogram"))
-        return DACH_CUDA_ERROR;
-    double t_reuse = 0;
-    auto issue_h2d = [&](size_t k) -> bool {
-        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
+    // the batch's histogram: zeroed before any slice adds into it (the slices run on the slots' streams)
+    auto zero_acc = [&]() -> int {
+        if (!ensure(acc, n_hist * 8) || !cuda_ok(cudaMemsetAsync(acc.p, 0, n_hist * 8, d->slot[0].stream), "memset histogram") ||
+            !cuda_ok(cudaStreamSynchronize(d->slot[0].stream), "memset histogram"))
+            return DACH_CUDA_ERROR;
+        return DACH_OK;
     };
-    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
-    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
     uint64_t sum = 0;
-    for (size_t k = 0; k < slices.size(); ++k) {
-        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
-        Workspace& W = d->slot[k % dach_dev::kSlots];
-        const Slice& s = slices[k];
-        const uint64_t tb = offs[s.last] - offs[s.first], ns = s.last - s.first;
-        const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
-        rc = enqueue_rk(d, W, RK_HIST, mode, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb, tb,
-                        static_cast<const uint64_t*>(W.offs.p), ns, nullptr, nullptr, nullptr, W.stream, key, static_cast<uint64_t*>(acc.p));
+    SliceRun run;
+    rc = run_slices(d, mode, text, offs, n, "scan", run, zero_acc, [&](size_t, const SliceOnSlot& x) -> int {
+        const RkOut o{.key = key, .hist = static_cast<uint64_t*>(acc.p)};
+        int r = enqueue_rk(d, x.W, RK_HIST, mode, x.d_text, x.lo(), x.end(), x.tb, x.d_offs(), x.ns, o, x.W.stream);
         uint64_t t = 0;
-        if (!rc) rc = finish_rk(d, W, &t);
-        if (rc) return rc;
+        if (!r) r = finish_rk(d, x.W, &t);
+        if (r) return r;
         sum += t;
-    }
-    for (Workspace& w : d->slot)
-        if (!cuda_ok(cudaStreamSynchronize(w.stream), "scan")) return DACH_CUDA_ERROR;
+        return DACH_OK;
+    });
+    if (rc) return rc;
     std::vector<uint64_t> h(n_hist);
     if (n_hist && !cuda_ok(cudaMemcpy(h.data(), acc.p, n_hist * 8, cudaMemcpyDeviceToHost), "D2H histogram")) return DACH_CUDA_ERROR;
     d->last_d2h = n_hist * 8;
@@ -2685,8 +2475,8 @@ int df_windows(dach_dev* d, Workspace& W, int mode, int key, const uint8_t* d_te
     for (uint64_t a = first; a < last;) {
         const uint64_t b = last - a <= *win ? last : a + *win;
         d->df_clean = false;
-        int rc = enqueue_rk(d, W, RK_DF, mode, d_text, text_lo, text_end, offs[b] - offs[a], d_offs + (a - first), b - a, nullptr, nullptr,
-                            nullptr, st, key, static_cast<uint64_t*>(d->df_acc.p));
+        const RkOut o{.key = key, .hist = static_cast<uint64_t*>(d->df_acc.p)};
+        int rc = enqueue_rk(d, W, RK_DF, mode, d_text, text_lo, text_end, offs[b] - offs[a], d_offs + (a - first), b - a, o, st);
         if (rc) return rc;
         d->df_clean = true;  // k_df_clear and the counters' reset are enqueued
         uint64_t t = 0;
@@ -2719,10 +2509,7 @@ int df_batch_dev_impl(dach_dev* d, int mode, int key, const uint8_t* d_text, con
     d->last_df_windows = d->last_df_rescans = 0;
     if (total) *total = 0;
     if (n == 0) return DACH_OK;
-    if (n > 0xfffffff0ull) {
-        set_error("too many haystacks in one batch (max 2^32-16)");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (n > 0xfffffff0ull) return invalid("too many haystacks in one batch (max 2^32-16)");
     std::vector<uint64_t> offs(n + 1);
     if (!cuda_ok(cudaMemcpyAsync(offs.data(), d_offs, (n + 1) * 8, cudaMemcpyDeviceToHost, st), "D2H offsets") ||
         !cuda_ok(cudaStreamSynchronize(st), "D2H offsets"))
@@ -2730,10 +2517,7 @@ int df_batch_dev_impl(dach_dev* d, int mode, int key, const uint8_t* d_text, con
     d->last_d2h = (n + 1) * 8;
     int rc = check_host_offsets(offs.data(), n);
     if (rc) return rc;
-    if (offs[n] > text_bytes) {
-        set_error("haystack offsets must be inside text_bytes");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (offs[n] > text_bytes) return invalid("haystack offsets must be inside text_bytes");
     rc = df_prepare(d, n_df, st);
     if (rc) return rc;
     const std::vector<Slice> slices = cut_slices(d, mode, offs.data(), n);
@@ -2757,10 +2541,7 @@ int df_batch_dev_impl(dach_dev* d, int mode, int key, const uint8_t* d_text, con
 // is added into the caller's
 int df_batch_host_impl(dach_dev* d, int mode, int key, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* df, uint64_t n_df,
                        uint64_t* total) {
-    if (!d || !offs || (n_df && !df)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!d || !offs || (n_df && !df)) return invalid("null argument");
     int rc = check_hist(d, key, n_df);
     if (rc) return rc;
     rc = check_mode(d, mode);
@@ -2772,39 +2553,13 @@ int df_batch_host_impl(dach_dev* d, int mode, int key, const uint8_t* text, cons
     d->last_df_windows = d->last_df_rescans = 0;
     if (total) *total = 0;
     if (n == 0) return DACH_OK;
-    rc = check_host_offsets(offs, n);
-    if (rc) return rc;
-    struct Drain {  // no exit may leave copies of the caller's buffers in flight
-        dach_dev* d;
-        ~Drain() {
-            for (Workspace& w : d->slot)
-                if (w.stream) cudaStreamSynchronize(w.stream);
-        }
-    } drain_on_exit{d};
-    const std::vector<Slice> slices = cut_slices(d, mode, offs, n);
-    for (Workspace& w : d->slot)
-        if (!w.init(true)) return DACH_CUDA_ERROR;
-    rc = df_prepare(d, n_df, d->slot[0].stream);
-    if (rc) return rc;
-    double t_reuse = 0;
-    auto issue_h2d = [&](size_t k) -> bool {
-        return slice_h2d(d, d->slot[k % dach_dev::kSlots], text, offs, slices[k].first, slices[k].last, &t_reuse);
-    };
-    if (!issue_h2d(0)) return DACH_CUDA_ERROR;
-    if (slices.size() > 1 && !issue_h2d(1)) return DACH_CUDA_ERROR;
     uint64_t win = ~0ull, sum = 0;
-    for (size_t k = 0; k < slices.size(); ++k) {
-        if (k + 2 < slices.size() && !issue_h2d(k + 2)) return DACH_CUDA_ERROR;
-        Workspace& W = d->slot[k % dach_dev::kSlots];
-        const Slice& s = slices[k];
-        const uint64_t tb = offs[s.last] - offs[s.first];
-        const uint8_t* d_text = static_cast<const uint8_t*>(W.text.p) - offs[s.first];
-        rc = df_windows(d, W, mode, key, d_text, static_cast<const uint8_t*>(W.text.p), static_cast<const uint8_t*>(W.text.p) + tb,
-                        static_cast<const uint64_t*>(W.offs.p), offs, s.first, s.last, W.stream, &win, &sum);
-        if (rc) return rc;
-    }
-    for (Workspace& w : d->slot)
-        if (!cuda_ok(cudaStreamSynchronize(w.stream), "scan")) return DACH_CUDA_ERROR;
+    SliceRun run;
+    rc = run_slices(d, mode, text, offs, n, "scan", run, [&]() { return df_prepare(d, n_df, d->slot[0].stream); },
+                    [&](size_t, const SliceOnSlot& x) -> int {
+        return df_windows(d, x.W, mode, key, x.d_text, x.lo(), x.end(), x.d_offs(), offs, x.s.first, x.s.last, x.W.stream, &win, &sum);
+    });
+    if (rc) return rc;
     std::vector<uint64_t> h(n_df);
     if (n_df && !cuda_ok(cudaMemcpy(h.data(), d->df_acc.p, n_df * 8, cudaMemcpyDeviceToHost), "D2H document frequencies"))
         return DACH_CUDA_ERROR;
@@ -2838,10 +2593,7 @@ extern "C" {
 int dach_dev_upload(const dach_pma* pma, int device, dach_dev** out) {
     if (!out) return DACH_INVALID_ARGUMENT;
     *out = nullptr;
-    if (!pma) {
-        set_error("null automaton");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!pma) return invalid("null automaton");
     return guarded([&]() -> int {
         HostImage img;
         if (const char* e = getenv("DACH_HOT_SLOTS")) img.want_hot_slots = (uint32_t)strtoul(e, nullptr, 10);  // layout experiments
@@ -2933,10 +2685,7 @@ size_t dach_dev_image_bytes(const dach_dev* d) { return d ? d->image_bytes : 0; 
 int dach_dev_scan_batch(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n,
                         uint64_t text_bytes, dach_match* d_out, uint64_t out_cap, uint64_t* d_out_offs,
                         uint64_t* needed, void* stream) {
-    if (!d || !d_offs || !d_out_offs || (out_cap && !d_out)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!d || !d_offs || !d_out_offs || (out_cap && !d_out)) return invalid("null argument");
     const int rc = check_mode(d, mode);
     if (rc) return rc;
     return guarded([&]() -> int {
@@ -2951,15 +2700,10 @@ int dach_dev_scan_batch(dach_dev* d, int mode, const uint8_t* d_text, const uint
 int dach_dev_scan_stream(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                          uint32_t* d_state, const uint32_t* d_pos, dach_match* d_out, uint64_t out_cap, uint64_t* d_out_offs,
                          uint64_t* needed, void* stream) {
-    if (!d || !d_offs || !d_out_offs || !d_state || (out_cap && !d_out)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    if (mode != DACH_FIND && mode != DACH_FIND_OVERLAPPING) {
-        set_error("stream chunks: mode must be DACH_FIND or DACH_FIND_OVERLAPPING (the crate's two steppers)");
-        return DACH_INVALID_ARGUMENT;
-    }
-    const int rc = check_mode(d, mode);
+    if (!d || !d_offs || !d_out_offs || !d_state || (out_cap && !d_out)) return invalid("null argument");
+    int rc = check_stream_mode(mode);
+    if (rc) return rc;
+    rc = check_mode(d, mode);
     if (rc) return rc;
     return guarded([&]() -> int {
         std::lock_guard<std::mutex> lk(d->mu);
@@ -2973,22 +2717,18 @@ int dach_dev_scan_stream(dach_dev* d, int mode, const uint8_t* d_text, const uin
 }  // extern "C"
 
 namespace {
-// COUNT / FIRST / HIST of stream chunks: the mode checks of dach_dev_scan_stream, then one enqueue_rk with the state
-int rk_stream(dach_dev* d, int rk, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
-              uint32_t* d_state, const uint32_t* d_pos, uint64_t* d_counts, dach_match* d_first, uint8_t* d_found, uint64_t* d_hist,
-              uint64_t* total, void* stream) {
-    if (mode != DACH_FIND && mode != DACH_FIND_OVERLAPPING) {
-        set_error("stream chunks: mode must be DACH_FIND or DACH_FIND_OVERLAPPING (the crate's two steppers)");
-        return DACH_INVALID_ARGUMENT;
-    }
+// COUNT / FIRST / HIST / MASK of a device batch or of stream chunks on the handle's workspace: the mode check, then
+// enqueue_rk under the handle's lock, then wait and report
+int rk_locked(dach_dev* d, int rk, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
+              const RkOut& o, uint64_t* total, void* stream) {
     const int rc = check_mode(d, mode);
     if (rc) return rc;
     return guarded([&]() -> int {
         std::lock_guard<std::mutex> lk(d->mu);
         DeviceGuard g(d->device);
         if (!g.ok) return DACH_CUDA_ERROR;
-        const int r = enqueue_rk(d, d->ws, rk, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, d_counts, d_first, d_found,
-                                 static_cast<cudaStream_t>(stream), key, d_hist, d_state, d_pos);
+        const int r = enqueue_rk(d, d->ws, rk, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, o,
+                                 static_cast<cudaStream_t>(stream));
         return r ? r : finish_rk(d, d->ws, total);
     });
 }
@@ -2998,31 +2738,27 @@ extern "C" {
 
 int dach_dev_count_stream(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                           uint32_t* d_state, uint64_t* d_counts, uint64_t* total, void* stream) {
-    if (!d || !d_offs || !d_state || (n && !d_counts)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    return rk_stream(d, RK_COUNT, mode, 0, d_text, d_offs, n, text_bytes, d_state, nullptr, d_counts, nullptr, nullptr, nullptr, total, stream);
+    if (!d || !d_offs || !d_state || (n && !d_counts)) return invalid("null argument");
+    const int rc = check_stream_mode(mode);
+    return rc ? rc : rk_locked(d, RK_COUNT, mode, d_text, d_offs, n, text_bytes, {.counts = d_counts, .state = d_state}, total, stream);
 }
 
 int dach_dev_first_stream(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                           uint32_t* d_state, const uint32_t* d_pos, dach_match* d_first, uint8_t* d_found, uint64_t* n_found, void* stream) {
-    if (!d || !d_offs || !d_state || (n && (!d_first || !d_found))) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    return rk_stream(d, RK_FIRST, mode, 0, d_text, d_offs, n, text_bytes, d_state, d_pos, nullptr, d_first, d_found, nullptr, n_found, stream);
+    if (!d || !d_offs || !d_state || (n && (!d_first || !d_found))) return invalid("null argument");
+    const RkOut o{.first = d_first, .found = d_found, .state = d_state, .pos = d_pos};
+    const int rc = check_stream_mode(mode);
+    return rc ? rc : rk_locked(d, RK_FIRST, mode, d_text, d_offs, n, text_bytes, o, n_found, stream);
 }
 
 int dach_dev_hist_stream(dach_dev* d, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                          uint32_t* d_state, uint64_t* d_hist, uint64_t n_hist, uint64_t* total, void* stream) {
-    if (!d || !d_offs || !d_state || (n_hist && !d_hist)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    const int rc = check_hist(d, key, n_hist);
+    if (!d || !d_offs || !d_state || (n_hist && !d_hist)) return invalid("null argument");
+    int rc = check_hist(d, key, n_hist);
     if (rc) return rc;
-    return rk_stream(d, RK_HIST, mode, key, d_text, d_offs, n, text_bytes, d_state, nullptr, nullptr, nullptr, nullptr, d_hist, total, stream);
+    rc = check_stream_mode(mode);
+    const RkOut o{.key = key, .hist = d_hist, .state = d_state};
+    return rc ? rc : rk_locked(d, RK_HIST, mode, d_text, d_offs, n, text_bytes, o, total, stream);
 }
 
 int dach_scan_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n,
@@ -3032,20 +2768,8 @@ int dach_scan_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint6
 
 int dach_dev_count_batch(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                          uint64_t* d_counts, uint64_t* total, void* stream) {
-    if (!d || !d_offs || (n && !d_counts)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    const int rc = check_mode(d, mode);
-    if (rc) return rc;
-    return guarded([&]() -> int {
-        std::lock_guard<std::mutex> lk(d->mu);
-        DeviceGuard g(d->device);
-        if (!g.ok) return DACH_CUDA_ERROR;
-        const int r = enqueue_rk(d, d->ws, RK_COUNT, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, d_counts, nullptr,
-                                 nullptr, static_cast<cudaStream_t>(stream));
-        return r ? r : finish_rk(d, d->ws, total);
-    });
+    if (!d || !d_offs || (n && !d_counts)) return invalid("null argument");
+    return rk_locked(d, RK_COUNT, mode, d_text, d_offs, n, text_bytes, {.counts = d_counts}, total, stream);
 }
 
 int dach_count_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* counts, uint64_t* total) {
@@ -3054,20 +2778,8 @@ int dach_count_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint
 
 int dach_dev_first_batch(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                          dach_match* d_first, uint8_t* d_found, uint64_t* n_found, void* stream) {
-    if (!d || !d_offs || (n && (!d_first || !d_found))) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    const int rc = check_mode(d, mode);
-    if (rc) return rc;
-    return guarded([&]() -> int {
-        std::lock_guard<std::mutex> lk(d->mu);
-        DeviceGuard g(d->device);
-        if (!g.ok) return DACH_CUDA_ERROR;
-        const int r = enqueue_rk(d, d->ws, RK_FIRST, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, nullptr, d_first,
-                                 d_found, static_cast<cudaStream_t>(stream));
-        return r ? r : finish_rk(d, d->ws, n_found);
-    });
+    if (!d || !d_offs || (n && (!d_first || !d_found))) return invalid("null argument");
+    return rk_locked(d, RK_FIRST, mode, d_text, d_offs, n, text_bytes, {.first = d_first, .found = d_found}, n_found, stream);
 }
 
 int dach_first_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, dach_match* first, uint8_t* found,
@@ -3077,22 +2789,9 @@ int dach_first_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint
 
 int dach_dev_hist_batch(dach_dev* d, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                         uint64_t* d_hist, uint64_t n_hist, uint64_t* total, void* stream) {
-    if (!d || !d_offs || (n_hist && !d_hist)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    int rc = check_hist(d, key, n_hist);
-    if (rc) return rc;
-    rc = check_mode(d, mode);
-    if (rc) return rc;
-    return guarded([&]() -> int {
-        std::lock_guard<std::mutex> lk(d->mu);
-        DeviceGuard g(d->device);
-        if (!g.ok) return DACH_CUDA_ERROR;
-        const int r = enqueue_rk(d, d->ws, RK_HIST, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, nullptr, nullptr,
-                                 nullptr, static_cast<cudaStream_t>(stream), key, d_hist);
-        return r ? r : finish_rk(d, d->ws, total);
-    });
+    if (!d || !d_offs || (n_hist && !d_hist)) return invalid("null argument");
+    const int rc = check_hist(d, key, n_hist);
+    return rc ? rc : rk_locked(d, RK_HIST, mode, d_text, d_offs, n, text_bytes, {.key = key, .hist = d_hist}, total, stream);
 }
 
 int dach_hist_batch_host(dach_dev* d, int mode, int key, const uint8_t* text, const uint64_t* offs, uint64_t n, uint64_t* hist,
@@ -3102,10 +2801,7 @@ int dach_hist_batch_host(dach_dev* d, int mode, int key, const uint8_t* text, co
 
 int dach_dev_df_batch(dach_dev* d, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                       uint64_t* d_df, uint64_t n_df, uint64_t* total, void* stream) {
-    if (!d || !d_offs || (n_df && !d_df)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!d || !d_offs || (n_df && !d_df)) return invalid("null argument");
     int rc = check_hist(d, key, n_df);
     if (rc) return rc;
     rc = check_mode(d, mode);
@@ -3129,22 +2825,9 @@ int dach_dev_last_df_windows(const dach_dev* d, uint64_t* windows, uint64_t* res
 
 int dach_dev_mask_batch(dach_dev* d, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                         uint8_t fill, uint8_t* d_out, void* stream) {
-    if (!d || !d_offs || (text_bytes && (!d_text || !d_out))) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    int rc = check_mask(d, d_text, text_bytes, fill, d_out);
-    if (rc) return rc;
-    rc = check_mode(d, mode);
-    if (rc) return rc;
-    return guarded([&]() -> int {
-        std::lock_guard<std::mutex> lk(d->mu);
-        DeviceGuard g(d->device);
-        if (!g.ok) return DACH_CUDA_ERROR;
-        const int r = enqueue_rk(d, d->ws, RK_MASK, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, nullptr, nullptr,
-                                 nullptr, static_cast<cudaStream_t>(stream), 0, nullptr, nullptr, nullptr, d_out, fill);
-        return r ? r : finish_rk(d, d->ws, nullptr);
-    });
+    if (!d || !d_offs || (text_bytes && (!d_text || !d_out))) return invalid("null argument");
+    const int rc = check_mask(d, d_text, text_bytes, fill, d_out);
+    return rc ? rc : rk_locked(d, RK_MASK, mode, d_text, d_offs, n, text_bytes, {.masked = d_out, .fill = fill}, nullptr, stream);
 }
 
 int dach_mask_batch_host(dach_dev* d, int mode, const uint8_t* text, const uint64_t* offs, uint64_t n, uint8_t fill, uint8_t* out) {
@@ -3166,25 +2849,19 @@ void job_time_zero(dach_dev* d, cudaStream_t stream) {
 // COUNT / FIRST / HIST / MASK on a job: the mode check of the synchronous call (the caller has made the others), then
 // enqueue_rk on the job's workspace, ordered after the job's previous operation; dach_job_wait reports it.  No handle
 // mutex and no handle-wide state: the job's own workspace, events and pinned block only.
-int job_rk(dach_job* j, int rk, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
-           uint64_t* d_counts, dach_match* d_first, uint8_t* d_found, uint64_t* d_hist, uint8_t* d_masked, uint8_t fill, void* stream) {
+int job_rk(dach_job* j, int rk, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes, const RkOut& o,
+           void* stream) {
     int rc = check_mode(j->d, mode);
     if (rc) return rc;
-    if (n > 0xfffffff0ull) {  // enqueue_rk's check, made here so that nothing at all is recorded on the stream
-        set_error("too many haystacks in one batch (max 2^32-16)");
-        return DACH_INVALID_ARGUMENT;
-    }
-    if (j->unplaced) {
-        set_error("the job's scan has not been placed (dach_job_place comes before the job's next operation)");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (n > 0xfffffff0ull)  // enqueue_rk's check, made here so that nothing at all is recorded on the stream
+        return invalid("too many haystacks in one batch (max 2^32-16)");
+    if (j->unplaced) return invalid("the job's scan has not been placed (dach_job_place comes before the job's next operation)");
     return guarded([&]() -> int {
         DeviceGuard g(j->d->device);
         if (!g.ok) return DACH_CUDA_ERROR;
         const cudaStream_t st = static_cast<cudaStream_t>(stream);
         job_time_zero(j->d, st);
-        const int r = enqueue_rk(j->d, j->W, rk, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, d_counts, d_first,
-                                 d_found, st, key, d_hist, nullptr, nullptr, d_masked, fill);
+        const int r = enqueue_rk(j->d, j->W, rk, mode, d_text, d_text, d_text + text_bytes, text_bytes, d_offs, n, o, st);
         if (r) return r;
         j->W.job_open = true;  // the job's next operation waits for W.ev_placed
         j->rk = rk;
@@ -3229,10 +2906,7 @@ void dach_job_free(dach_job* j) {
 
 int dach_job_scan(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                   uint64_t cap_matches, void* stream) {
-    if (!j || !d_offs) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!j || !d_offs) return invalid("null argument");
     const int rc = check_mode(j->d, mode);
     if (rc) return rc;
     return guarded([&]() -> int {
@@ -3250,14 +2924,8 @@ int dach_job_scan(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* 
 }
 
 int dach_job_place(dach_job* j, dach_match* d_out, uint64_t out_cap, uint64_t* d_out_offs, const uint64_t* d_base, void* stream) {
-    if (!j || !d_out_offs || (out_cap && !d_out)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    if (j->rk != RK_MATCHES) {
-        set_error("no scan to place: the job's last operation was a count, first-match, histogram or mask");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!j || !d_out_offs || (out_cap && !d_out)) return invalid("null argument");
+    if (j->rk != RK_MATCHES) return invalid("no scan to place: the job's last operation was a count, first-match, histogram or mask");
     return guarded([&]() -> int {
         DeviceGuard g(j->d->device);
         if (!g.ok) return DACH_CUDA_ERROR;
@@ -3271,60 +2939,41 @@ int dach_job_place(dach_job* j, dach_match* d_out, uint64_t out_cap, uint64_t* d
 
 int dach_job_count(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                    uint64_t* d_counts, void* stream) {
-    if (!j || !d_offs || (n && !d_counts)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    return job_rk(j, RK_COUNT, mode, 0, d_text, d_offs, n, text_bytes, d_counts, nullptr, nullptr, nullptr, nullptr, 0, stream);
+    if (!j || !d_offs || (n && !d_counts)) return invalid("null argument");
+    return job_rk(j, RK_COUNT, mode, d_text, d_offs, n, text_bytes, {.counts = d_counts}, stream);
 }
 
 int dach_job_first(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                    dach_match* d_first, uint8_t* d_found, void* stream) {
-    if (!j || !d_offs || (n && (!d_first || !d_found))) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
-    return job_rk(j, RK_FIRST, mode, 0, d_text, d_offs, n, text_bytes, nullptr, d_first, d_found, nullptr, nullptr, 0, stream);
+    if (!j || !d_offs || (n && (!d_first || !d_found))) return invalid("null argument");
+    return job_rk(j, RK_FIRST, mode, d_text, d_offs, n, text_bytes, {.first = d_first, .found = d_found}, stream);
 }
 
 int dach_job_hist(dach_job* j, int mode, int key, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes,
                   uint64_t* d_hist, uint64_t n_hist, void* stream) {
-    if (!j || !d_offs || (n_hist && !d_hist)) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!j || !d_offs || (n_hist && !d_hist)) return invalid("null argument");
     const int rc = check_hist(j->d, key, n_hist);
-    if (rc) return rc;
-    return job_rk(j, RK_HIST, mode, key, d_text, d_offs, n, text_bytes, nullptr, nullptr, nullptr, d_hist, nullptr, 0, stream);
+    return rc ? rc : job_rk(j, RK_HIST, mode, d_text, d_offs, n, text_bytes, {.key = key, .hist = d_hist}, stream);
 }
 
 int dach_job_mask(dach_job* j, int mode, const uint8_t* d_text, const uint64_t* d_offs, uint64_t n, uint64_t text_bytes, uint8_t fill,
                   uint8_t* d_out, void* stream) {
-    if (!j || !d_offs || (text_bytes && (!d_text || !d_out))) {
-        set_error("null argument");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!j || !d_offs || (text_bytes && (!d_text || !d_out))) return invalid("null argument");
     const int rc = check_mask(j->d, d_text, text_bytes, fill, d_out);
-    if (rc) return rc;
-    return job_rk(j, RK_MASK, mode, 0, d_text, d_offs, n, text_bytes, nullptr, nullptr, nullptr, nullptr, d_out, fill, stream);
+    return rc ? rc : job_rk(j, RK_MASK, mode, d_text, d_offs, n, text_bytes, {.masked = d_out, .fill = fill}, stream);
 }
 
 int dach_job_wait(dach_job* j, uint64_t* needed) {
     if (!j) return DACH_INVALID_ARGUMENT;
-    if (j->unplaced) {  // the last placement's report would be stale
-        set_error("dach_job_wait: the job's scan has not been placed yet");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (j->unplaced)  // the last placement's report would be stale
+        return invalid("dach_job_wait: the job's scan has not been placed yet");
     if (j->rk != RK_MATCHES)  // a reduction: *needed = its total (0 for MASK, whose total stays at its zero)
         return guarded([&]() -> int {
             DeviceGuard g(j->d->device);
             if (!g.ok) return DACH_CUDA_ERROR;
             return finish_rk(nullptr, j->W, needed);
         });
-    if (!j->W.job_placed) {
-        set_error("dach_job_wait: nothing has been placed yet");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!j->W.job_placed) return invalid("dach_job_wait: nothing has been placed yet");
     return guarded([&]() -> int {
         DeviceGuard g(j->d->device);
         if (!g.ok) return DACH_CUDA_ERROR;
@@ -3390,10 +3039,8 @@ static_assert(sizeof(GroupHandle) <= DACH_GROUP_HANDLE_BYTES, "DACH_GROUP_HANDLE
 int dach_group_create(int rank, int world, int device, uint64_t match_cap, uint64_t n_haystacks_total, dach_group** out) {
     if (!out) return DACH_INVALID_ARGUMENT;
     *out = nullptr;
-    if (world < 1 || world > kMaxRanks || rank < 0 || rank >= world) {
-        set_error("shard group: rank / world out of range (at most 16 ranks)");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (world < 1 || world > kMaxRanks || rank < 0 || rank >= world)
+        return invalid("shard group: rank / world out of range (at most 16 ranks)");
     return guarded([&]() -> int {
         DeviceGuard g(device);
         if (!g.ok) return DACH_CUDA_ERROR;
@@ -3475,10 +3122,7 @@ int dach_group_connect(dach_group* G, const void* handles) {
         for (int j = 0; j < G->world; ++j) {
             GroupHandle h;
             memcpy(&h, static_cast<const char*>(handles) + (size_t)j * DACH_GROUP_HANDLE_BYTES, sizeof(h));
-            if (h.rank != j) {
-                set_error("shard group: handles must be in rank order");
-                return DACH_INVALID_ARGUMENT;
-            }
+            if (h.rank != j) return invalid("shard group: handles must be in rank order");
             if (j == G->rank) {
                 G->peers.ctl[j] = G->ctl;
             } else {
@@ -3499,27 +3143,15 @@ int dach_group_connect(dach_group* G, const void* handles) {
 }
 
 int dach_group_place(dach_group* G, dach_job* j, uint64_t hay_base, int last, void* stream) {
-    if (!G || !j || !G->connected) {
-        set_error("shard group: not connected");
-        return DACH_INVALID_ARGUMENT;
-    }
-    if (j->rk != RK_MATCHES) {
-        set_error("no scan to place: the job's last operation was a count, first-match, histogram or mask");
-        return DACH_INVALID_ARGUMENT;
-    }
-    if (hay_base + j->W.job_n > G->n_total) {
-        set_error("shard group: haystack range outside the gathered batch");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!G || !j || !G->connected) return invalid("shard group: not connected");
+    if (j->rk != RK_MATCHES) return invalid("no scan to place: the job's last operation was a count, first-match, histogram or mask");
+    if (hay_base + j->W.job_n > G->n_total) return invalid("shard group: haystack range outside the gathered batch");
     return guarded([&]() -> int {
         DeviceGuard g(G->device);
         if (!g.ok) return DACH_CUDA_ERROR;
         cudaStream_t st = static_cast<cudaStream_t>(stream);
         Workspace& W = j->W;
-        if (!W.job_open) {
-            set_error("no scan to place");
-            return DACH_INVALID_ARGUMENT;
-        }
+        if (!W.job_open) return invalid("no scan to place");
         const unsigned long long step = ++G->step;
         if (st != W.job_stream) cudaStreamWaitEvent(st, W.ev_scanned, 0);
         // calling for step s says the result of step s-1 has been consumed: its buffers are free again
@@ -3590,10 +3222,7 @@ int dach_group_finish(dach_group* G, uint64_t* total, void* stream) {
 }
 
 int dach_group_result(const dach_group* G, dach_match** d_out, uint64_t** d_offs) {
-    if (!G || G->rank != 0) {
-        set_error("shard group: only the gathering rank (0) holds the result");
-        return DACH_INVALID_ARGUMENT;
-    }
+    if (!G || G->rank != 0) return invalid("shard group: only the gathering rank (0) holds the result");
     if (d_out) *d_out = G->out;
     if (d_offs) *d_offs = G->offs;
     return DACH_OK;

@@ -13,6 +13,7 @@
 #include "../../daachorse_b200/csrc/dev_image.h"
 #include "../../daachorse_b200/csrc/host.h"
 #include "../../daachorse_b200/csrc/scan_lane.cuh"
+#include "../../daachorse_b200/csrc/scan_plan.h"
 
 using namespace dach;
 
@@ -250,11 +251,16 @@ extern "C" int emu_scan_batch_wire(const uint8_t* wire, size_t wire_len, int cha
     if (rc) return rc;
     if ((mode == M_LEFTMOST) != lm) return DACH_MATCH_KIND_MISMATCH;
 
+    // kernel choice as enqueue_scan (one CTA per SM; StdMachine3's event queue and direct paths run the same lanes here)
+    // seg_len > 0 cuts even an automaton the device scans whole (not segmentable): the hand-made case of
+    // test_emu_lane.py shows with it why the device does not
+    const ScanPlan plan = plan_scan({.opt_kernel = kernel_version, .compact = !img.crec.empty(),
+                                     .charwise = charwise != 0, .root_opos = img.root_opos != 0,
+                                     .root_base = img.root_base != 0, .segmentable = true, .opt_seg_len = seg_len,
+                                     .stream = g_state_io != nullptr, .mode = mode});
+    if (plan.refused) return DACH_INVALID_ARGUMENT;
     // segment table (mirrors k_seg_count / k_seg_fill in dev_scan.cu)
-    const bool v1 = kernel_version >= 1 && !img.crec.empty() && !(mode == M_FIND && img.root_opos != 0);
-    if (g_state_io && !(v1 && mode != M_LEFTMOST && (charwise || (kernel_version >= 2 && img.root_base != 0))))
-        return DACH_INVALID_ARGUMENT;  // as scan_locked() in dev_scan.cu
-    const bool seg = v1 && !charwise && !g_state_io && seg_len > 0 && (mode == M_OVERLAPPING || mode == M_NO_SUFFIX);
+    const bool seg = plan.seg && seg_len > 0;
     std::vector<uint32_t> item_hay, item_beg;
     std::vector<uint64_t> seg_first(n + 1, 0);
     uint64_t n_items = n;
@@ -314,10 +320,11 @@ extern "C" int emu_scan_batch_wire(const uint8_t* wire, size_t wire_len, int cha
     RecView V{P.rec, reinterpret_cast<const uint4*>(hot.data()), hot_n, img.root_table.data()};
     const uint8_t* lo = text + (n ? offs[0] : 0);
     const uint8_t* hi = text + (n ? offs[n] : 0);
-    if (v1) {
+    const Machine m = plan.machine;
+    if (m != Machine::Lane) {
         // StdMachine3: the leading hot_n compact records are served from a "shared memory" copy; everything past
         // them in that copy is poison, so a wrong prefix compare cannot go unnoticed
-        uint32_t entries = (mode == M_LEFTMOST || charwise || kernel_version < 3) ? 0 : hot_n;
+        uint32_t entries = plan.std3() ? hot_n : 0;
         if (entries > img.hot_slots) entries = img.hot_slots;
         std::vector<uint32_t> tab(img.crec.size() ? img.crec.size() : 4, 0xdeadbeefu);
         memcpy(tab.data(), img.crec.data(), (size_t)entries * 16);
@@ -325,35 +332,43 @@ extern "C" int emu_scan_batch_wire(const uint8_t* wire, size_t wire_len, int cha
                   img.opos_tab.data(), P.text_end, P.text_lo, img.root_base, P.root_opos ? CF_OUT : 0u, nullptr, 0, 0, P.mapper, P.mapper_len,
                   reinterpret_cast<const uint4*>(img.crec.data())[D_ROOT]};
         const int n_warps = 3;
-        if (charwise) {
-            if (getenv("DACH_EMU_TRACE")) fprintf(stderr, "emu: charwise lane machine\n");
-            if (mode == M_FIND) run_machine<CwMachine<M_FIND>, LaneCw>(P, Ev, lo, n_warps);
-            if (mode == M_OVERLAPPING) run_machine<CwMachine<M_OVERLAPPING>, LaneCw>(P, Ev, lo, n_warps);
-            if (mode == M_NO_SUFFIX) run_machine<CwMachine<M_NO_SUFFIX>, LaneCw>(P, Ev, lo, n_warps);
-            if (mode == M_LEFTMOST) run_machine<CwMachine<M_LEFTMOST>, LaneCw>(P, Ev, lo, n_warps);
-        } else if (mode != M_LEFTMOST && kernel_version >= 4 && img.root_base != 0) {
-            if (getenv("DACH_EMU_TRACE")) fprintf(stderr, "emu: StdMachine3, two haystacks per lane\n");
-            Ev.hot_n = 0;
-            if (mode == M_FIND) run_duo<M_FIND>(P, Ev, n_warps);
-            if (mode == M_OVERLAPPING) run_duo<M_OVERLAPPING>(P, Ev, n_warps);
-            if (mode == M_NO_SUFFIX) run_duo<M_NO_SUFFIX>(P, Ev, n_warps);
-        } else if (mode != M_LEFTMOST && kernel_version >= 3 && img.root_base != 0) {
-            if (getenv("DACH_EMU_TRACE")) fprintf(stderr, "emu: StdMachine3, %u hot records\n", entries);
-            if (mode == M_FIND) run_machine<StdMachine3<M_FIND>, Lane3>(P, Ev, lo, n_warps);
-            if (mode == M_OVERLAPPING) run_machine<StdMachine3<M_OVERLAPPING>, Lane3>(P, Ev, lo, n_warps);
-            if (mode == M_NO_SUFFIX) run_machine<StdMachine3<M_NO_SUFFIX>, Lane3>(P, Ev, lo, n_warps);
-        } else if (mode != M_LEFTMOST && kernel_version >= 2 && img.root_base != 0) {
-            if (getenv("DACH_EMU_TRACE")) fprintf(stderr, "emu: StdMachine2\n");
-            if (mode == M_FIND) run_machine<StdMachine2<M_FIND>, Lane2>(P, Ev, lo, n_warps);
-            if (mode == M_OVERLAPPING) run_machine<StdMachine2<M_OVERLAPPING>, Lane2>(P, Ev, lo, n_warps);
-            if (mode == M_NO_SUFFIX) run_machine<StdMachine2<M_NO_SUFFIX>, Lane2>(P, Ev, lo, n_warps);
-        } else if (mode == M_LEFTMOST) {
-            if (getenv("DACH_EMU_TRACE")) fprintf(stderr, "emu: leftmost lane machine\n");
-            run_machine<LmMachine, LaneLm>(P, Ev, lo, n_warps);
-        } else {
-            if (mode == M_FIND) run_items_v1<M_FIND>(P, Ev, lo, n_warps);
-            if (mode == M_OVERLAPPING) run_items_v1<M_OVERLAPPING>(P, Ev, lo, n_warps);
-            if (mode == M_NO_SUFFIX) run_items_v1<M_NO_SUFFIX>(P, Ev, lo, n_warps);
+        const bool trace = getenv("DACH_EMU_TRACE") != nullptr;
+        switch (m) {
+            case Machine::Cw:
+                if (trace) fprintf(stderr, "emu: charwise lane machine\n");
+                if (mode == M_FIND) run_machine<CwMachine<M_FIND>, LaneCw>(P, Ev, lo, n_warps);
+                if (mode == M_OVERLAPPING) run_machine<CwMachine<M_OVERLAPPING>, LaneCw>(P, Ev, lo, n_warps);
+                if (mode == M_NO_SUFFIX) run_machine<CwMachine<M_NO_SUFFIX>, LaneCw>(P, Ev, lo, n_warps);
+                if (mode == M_LEFTMOST) run_machine<CwMachine<M_LEFTMOST>, LaneCw>(P, Ev, lo, n_warps);
+                break;
+            case Machine::Duo:
+                if (trace) fprintf(stderr, "emu: StdMachine3, two haystacks per lane\n");
+                Ev.hot_n = 0;
+                if (mode == M_FIND) run_duo<M_FIND>(P, Ev, n_warps);
+                if (mode == M_OVERLAPPING) run_duo<M_OVERLAPPING>(P, Ev, n_warps);
+                if (mode == M_NO_SUFFIX) run_duo<M_NO_SUFFIX>(P, Ev, n_warps);
+                break;
+            case Machine::Std3:
+            case Machine::Std3Direct:
+                if (trace) fprintf(stderr, "emu: StdMachine3, %u hot records\n", entries);
+                if (mode == M_FIND) run_machine<StdMachine3<M_FIND>, Lane3>(P, Ev, lo, n_warps);
+                if (mode == M_OVERLAPPING) run_machine<StdMachine3<M_OVERLAPPING>, Lane3>(P, Ev, lo, n_warps);
+                if (mode == M_NO_SUFFIX) run_machine<StdMachine3<M_NO_SUFFIX>, Lane3>(P, Ev, lo, n_warps);
+                break;
+            case Machine::Std2:
+                if (trace) fprintf(stderr, "emu: StdMachine2\n");
+                if (mode == M_FIND) run_machine<StdMachine2<M_FIND>, Lane2>(P, Ev, lo, n_warps);
+                if (mode == M_OVERLAPPING) run_machine<StdMachine2<M_OVERLAPPING>, Lane2>(P, Ev, lo, n_warps);
+                if (mode == M_NO_SUFFIX) run_machine<StdMachine2<M_NO_SUFFIX>, Lane2>(P, Ev, lo, n_warps);
+                break;
+            case Machine::Lm:
+                if (trace) fprintf(stderr, "emu: leftmost lane machine\n");
+                run_machine<LmMachine, LaneLm>(P, Ev, lo, n_warps);
+                break;
+            default:
+                if (mode == M_FIND) run_items_v1<M_FIND>(P, Ev, lo, n_warps);
+                if (mode == M_OVERLAPPING) run_items_v1<M_OVERLAPPING>(P, Ev, lo, n_warps);
+                if (mode == M_NO_SUFFIX) run_items_v1<M_NO_SUFFIX>(P, Ev, lo, n_warps);
         }
     } else
     switch ((charwise ? 4 : 0) + mode) {

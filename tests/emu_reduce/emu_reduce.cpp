@@ -16,6 +16,7 @@
 #include "../../daachorse_b200/csrc/dev_image.h"
 #include "../../daachorse_b200/csrc/host.h"
 #include "../../daachorse_b200/csrc/scan_lane.cuh"
+#include "../../daachorse_b200/csrc/scan_plan.h"
 
 using namespace dach;
 
@@ -180,13 +181,14 @@ extern "C" int emu_reduce_batch_wire(const uint8_t* wire, size_t wire_len, int c
     if (mode < M_FIND || mode > M_LEFTMOST || (rk != RK_COUNT && rk != RK_FIRST)) return DACH_INVALID_ARGUMENT;
     if ((mode == M_LEFTMOST) != lm) return DACH_MATCH_KIND_MISMATCH;
     // kernel choice and segments as enqueue_rk
-    const int mmode = (rk == RK_FIRST && mode != M_LEFTMOST) ? M_OVERLAPPING : mode;
-    const bool v1 = kernel >= 1 && !img.crec.empty() && !(mmode == M_FIND && img.root_opos != 0);
-    const bool cw_machine = v1 && charwise;
-    const bool lm_machine = v1 && !charwise && mmode == M_LEFTMOST;
-    const bool std3 = v1 && !charwise && mmode != M_LEFTMOST && img.root_base != 0;
-    const int which = std3 ? 3 : (cw_machine || lm_machine) ? 1 : 0;
-    const bool seg = std3 && seg_len > 0 && (mmode == M_OVERLAPPING || mmode == M_NO_SUFFIX);
+    const ScanPlan plan = plan_scan({.opt_kernel = kernel, .compact = !img.crec.empty(), .charwise = charwise != 0,
+                                     .root_opos = img.root_opos != 0, .root_base = img.root_base != 0,
+                                     .segmentable = img.segmentable, .matches = false, .first = rk == RK_FIRST,
+                                     .mode = mode});
+    const int mmode = plan.mode;
+    const bool machine = plan.lane_machine();
+    const int which = plan.machine == Machine::Std3 ? 3 : machine ? 1 : 0;
+    const bool seg = plan.seg && seg_len > 0;
     std::vector<uint32_t> item_hay, item_beg;
     std::vector<uint64_t> seg_first(n + 1, 0);
     uint64_t n_items = n;
@@ -243,7 +245,7 @@ extern "C" int emu_reduce_batch_wire(const uint8_t* wire, size_t wire_len, int c
     std::vector<uint32_t> tab(img.crec.size() ? img.crec.size() : 4, 0xdeadbeefu);
     if (entries) memcpy(tab.data(), img.crec.data(), (size_t)entries * 16);
     StdEnv Ev{};
-    if (v1)
+    if (machine)
         Ev = StdEnv{reinterpret_cast<const uint4*>(img.crec.data()), reinterpret_cast<const uint4*>(tab.data()), 0u, entries,
                     img.opos_tab.data(), P.text_end, P.text_lo, img.root_base, P.root_opos ? CF_OUT : 0u, nullptr, 0, 0, P.mapper,
                     P.mapper_len, reinterpret_cast<const uint4*>(img.crec.data())[D_ROOT]};

@@ -17,6 +17,7 @@
 #include "../../daachorse_b200/csrc/dev_image.h"
 #include "../../daachorse_b200/csrc/host.h"
 #include "../../daachorse_b200/csrc/scan_lane.cuh"
+#include "../../daachorse_b200/csrc/scan_plan.h"
 
 using namespace dach;
 
@@ -163,10 +164,12 @@ extern "C" int emu_rk_stream_wire(const uint8_t* wire, size_t wire_len, int char
     if (total) *total = 0;
     if (n == 0) return DACH_OK;
     // the refusal of enqueue_rk / enqueue_scan: stream chunks need a Standard lane machine
-    const bool v1 = kernel >= 1 && !img.crec.empty() && !(mode == M_FIND && img.root_opos != 0);
-    const bool cw_machine = v1 && charwise;
-    const bool std3 = v1 && !charwise && img.root_base != 0;
-    if (!std3 && !cw_machine) return DACH_INVALID_ARGUMENT;
+    const ScanPlan plan = plan_scan({.opt_kernel = kernel, .compact = !img.crec.empty(), .charwise = charwise != 0,
+                                     .root_opos = img.root_opos != 0, .root_base = img.root_base != 0,
+                                     .segmentable = img.segmentable, .stream = true, .matches = false,
+                                     .first = rk == RK_FIRST, .mode = mode});
+    if (plan.refused) return DACH_INVALID_ARGUMENT;
+    const bool std3 = plan.machine == Machine::Std3;
     const uint32_t n_cslots = (uint32_t)img.opos_tab.size();
     std::vector<unsigned long long> item_count(n, 0), slot_hist(n_cslots + 1, 0), rec_hist(n_out + 1, 0);
     std::vector<uint4> item_first(n);
