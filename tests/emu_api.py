@@ -1,5 +1,6 @@
-"""ctypes binding of tests/emu/libdach_emu.so: the kernels' lane logic compiled for the CPU
-(test infrastructure only)."""
+"""ctypes binding of tests/emu/libdach_emu.so: the kernels' lane logic compiled for the CPU, every result kind
+(test infrastructure only).  The library is built and loaded here once; emu_reduce_api, emu_hist_api, emu_df_api,
+emu_mask_api and emu_events_api wrap its other entry points."""
 import ctypes as C
 import os
 import subprocess
@@ -12,32 +13,66 @@ LIB = os.path.join(EMU_DIR, "libdach_emu.so")
 MATCH_DTYPE = np.dtype([("start", "<u4"), ("end", "<u4"), ("value", "<u4")])
 _lib = None
 
+_P, _SZ, _I, _U32, _U64, _I64 = C.c_void_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint64, C.c_int64
+_PU32, _PU64, _PI = C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_int)
+_SIGNATURES = {  # name: (restype, argtypes)
+    "emu_scan_batch_wire": (_I, [_P, _SZ, _I, _I, _P, _P, _U64, _U32, _I, _U32, _U32, _U32, _P, _U64, _P, _PU64]),
+    "emu_scan_stream_wire": (_I, [_P, _SZ, _I, _P, _P, _U64, _P, _P, _U32, _P, _U64, _P, _PU64]),
+    "emu_events_scan_wire": (_I, [_P, _SZ, _I, _P, _P, _U64, _U32, _U32, _U32, _U32, _P, _P, _P, _U64, _P, _PU64, _PU32,
+                                  _I, _U32, _U32]),
+    "emu_place_tables": (_I64, [_P, _SZ, _P, _P, _U64]),
+    "emu_reduce_batch_wire": (_I, [_P, _SZ, _I, _I, _I, _P, _P, _U64, _U32, _I, _U32, _P, _P, _P, _PU64]),
+    "emu_rk_stream_wire": (_I, [_P, _SZ, _I, _I, _I, _I, _P, _P, _U64, _P, _P, _U32, _I, _I64, _P, _P, _P, _P, _U64, _PU64]),
+    "emu_hist_batch_wire": (_I, [_P, _SZ, _I, _I, _I, _P, _P, _U64, _U32, _I, _U32, _I64, _P, _U64, _PU64, _PI]),
+    "emu_hist_event_shares": (_I, [_P, _SZ, _I, _I, _P, _P, _U64, _P, _I, _P]),
+    "emu_df_batch_wire": (_I, [_P, _SZ, _I, _I, _I, _P, _P, _U64, _U32, _I, _U32, _I64, _I, _P, _U64, _PU64, _P]),
+    "emu_mask_batch_wire": (_I, [_P, _SZ, _I, _I, _P, _P, _U64, _U64, C.c_uint8, _U32, _I, _U32, _P, _PI]),
+    "emu_check_image_transitions": (C.c_longlong, [_P, _SZ, _U32, _PU32, _PU32]),
+    "emu_check_image_transitions_charwise": (C.c_longlong, [_P, _SZ]),
+    "emu_image_segmentable": (_I, [_P, _SZ]),
+    "emu_image_outputs": (C.c_longlong, [_P, _SZ, _I, _P, _SZ]),
+    "emu_stats": (None, [_P, _I]),
+    "emu_set_hot_slots": (None, [_U32]),
+    "emu_stream_config": (None, [_I, _U32]),
+    "emu_stream_charwise": (None, [_I]),
+}
+
 
 def lib():
     global _lib
     if _lib is None:
         subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
-        _lib = C.CDLL(LIB)
-        _lib.emu_scan_batch_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                             C.c_uint64, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
-                                             C.c_void_p, C.POINTER(C.c_uint64)]
-        _lib.emu_scan_batch_wire.restype = C.c_int
-        _lib.emu_scan_stream_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
-                                              C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]
-        _lib.emu_scan_stream_wire.restype = C.c_int
-        _lib.emu_check_image_transitions.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, C.POINTER(C.c_uint32),
-                                                     C.POINTER(C.c_uint32)]
-        _lib.emu_check_image_transitions.restype = C.c_longlong
-        _lib.emu_check_image_transitions_charwise.argtypes = [C.c_void_p, C.c_size_t]
-        _lib.emu_check_image_transitions_charwise.restype = C.c_longlong
+        L = C.CDLL(LIB)
+        for name, (res, args) in _SIGNATURES.items():
+            f = getattr(L, name)
+            f.restype, f.argtypes = res, args
+        _lib = L
     return _lib
+
+
+def stats(reset=True):
+    """EmuStats of the lane machines since the last reset: dict with 'steps', 'probes', ..."""
+    names = ("steps", "probes", "hits", "miss_known", "miss_f2root", "learns", "root_falls", "root_stay", "sig_skips",
+             "pushes", "cache_hits")
+    buf = (C.c_ulonglong * len(names))()
+    lib().emu_stats(buf, int(reset))
+    return dict(zip(names, list(buf)))
 
 
 def image_segmentable(wire):
     """HostImage::segmentable of a serialized bytewise automaton (1 / 0; -1: refused)."""
     wire_a = np.frombuffer(wire, dtype=np.uint8)
-    lib().emu_image_segmentable.argtypes = [C.c_void_p, C.c_size_t]
     return int(lib().emu_image_segmentable(wire_a.ctypes.data, wire_a.size))
+
+
+def image_outputs(wire, charwise=False):
+    """The device image's output records as an (k, 4) uint32 array {value, length, parent, chain}."""
+    L = lib()
+    wire_a = np.frombuffer(wire, dtype=np.uint8)
+    k = L.emu_image_outputs(wire_a.ctypes.data, wire_a.size, int(charwise), None, 0)
+    out = np.zeros((max(k, 1), 4), dtype=np.uint32)
+    L.emu_image_outputs(wire_a.ctypes.data, wire_a.size, int(charwise), out.ctypes.data, k)
+    return out[:k]
 
 
 def check_image_transitions_charwise(wire):

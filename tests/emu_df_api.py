@@ -1,29 +1,12 @@
-"""ctypes binding of tests/emu_df/libdach_emu_df.so: per-pattern document frequencies (dach_dev_df_batch) on the kernels'
-lane logic compiled for the CPU (test infrastructure only)."""
+"""Per-pattern document frequencies (dach_dev_df_batch) on the CPU emulation of the kernels' lane logic,
+tests/emu/libdach_emu.so (test infrastructure only)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-EMU_DIR = os.path.join(_HERE, "emu_df")
-LIB = os.path.join(EMU_DIR, "libdach_emu_df.so")
+from emu_api import lib
+
 KEY = {"output": 0, "value": 1}
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
-        L = C.CDLL(LIB)
-        L.emu_df_batch_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
-                                        C.c_uint32, C.c_int, C.c_uint32, C.c_int64, C.c_int, C.c_void_p, C.c_uint64,
-                                        C.POINTER(C.c_uint64), C.c_void_p]
-        L.emu_df_batch_wire.restype = C.c_int
-        _lib = L
-    return _lib
 
 
 def df(wire, charwise, mode, key, text, offs, n_df, hot_n=0, kernel=3, seg_len=0, df_pairs=1 << 16, split=True, out=None):

@@ -1,35 +1,21 @@
-"""ctypes binding of tests/emu_events/libdach_emu_events.so: StdMachine3's matches path with event blocks (the drain
-that stores events, k_expand) on the kernels' lane logic compiled for the CPU (test infrastructure only)."""
+"""StdMachine3's matches path with event blocks on the CPU emulation of the kernels' lane logic,
+tests/emu/libdach_emu.so (test infrastructure only): the queue kernel or the direct one, placed by k_expand or
+by block descriptors (k_blk_desc / k_expand_desc)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-EMU_DIR = os.path.join(_HERE, "emu_events")
-LIB = os.path.join(EMU_DIR, "libdach_emu_events.so")
-MATCH_DTYPE = np.dtype([("start", "<u4"), ("end", "<u4"), ("value", "<u4")])
+from emu_api import MATCH_DTYPE, lib  # noqa: F401
+
 NOT_STD3 = -1  # the automaton or mode does not run on StdMachine3
-_lib = None
 
 
-def lib():
-    global _lib
-    if _lib is None:
-        subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
-        L = C.CDLL(LIB)
-        L.emu_events_scan_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
-                                           C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
-                                           C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
-        L.emu_events_scan_wire.restype = C.c_int
-        _lib = L
-    return _lib
-
-
-def scan(wire, mode, text, offs, hot_n=0, seg_len=0, seg_from=0, pool_blocks=None, out_cap=None, state=None, pos=None):
+def scan(wire, mode, text, offs, hot_n=0, seg_len=0, seg_from=0, pool_blocks=None, out_cap=None, state=None, pos=None,
+         direct=False, place_u=0, place_pad=0):
     """Returns (rc, matches, out_offs, needed, blocks_used).  Without pool_blocks / out_cap both grow until the batch
-    fits.  `state` (np.uint32, n): stream chunks, updated in place; `pos` (np.uint32, n): their first positions."""
+    fits.  `state` (np.uint32, n): stream chunks, updated in place; `pos` (np.uint32, n): their first positions.
+    direct: k_scan_direct instead of the queue kernel; place_u > 0: placed from block descriptors (k_expand_desc),
+    place_u blocks per warp, the output place_pad words past a 16-byte boundary."""
     wire_a = np.frombuffer(wire, dtype=np.uint8)
     text = np.ascontiguousarray(text, dtype=np.uint8)
     offs = np.ascontiguousarray(offs, dtype=np.uint64)
@@ -45,7 +31,7 @@ def scan(wire, mode, text, offs, hot_n=0, seg_len=0, seg_from=0, pool_blocks=Non
         rc = lib().emu_events_scan_wire(wire_a.ctypes.data, wire_a.size, mode, pad.ctypes.data, offs.ctypes.data, n, hot_n,
                                         seg_len, seg_from, pb, state.ctypes.data if state is not None else None,
                                         pos.ctypes.data if pos is not None else None, out.ctypes.data, cap, oo.ctypes.data,
-                                        C.byref(need), C.byref(used))
+                                        C.byref(need), C.byref(used), int(direct), place_u, place_pad)
         if rc == 6 and out_cap is None and pool_blocks is None:
             if state is not None:
                 state[:] = saved

@@ -1,33 +1,12 @@
-"""ctypes binding of tests/emu_hist/libdach_emu_hist.so: per-pattern histograms (dach_dev_hist_batch) on the kernels'
-lane logic compiled for the CPU (test infrastructure only)."""
+"""Per-pattern histograms (dach_dev_hist_batch) on the CPU emulation of the kernels' lane logic,
+tests/emu/libdach_emu.so (test infrastructure only)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-EMU_DIR = os.path.join(_HERE, "emu_hist")
-LIB = os.path.join(EMU_DIR, "libdach_emu_hist.so")
+from emu_api import lib
+
 KEY = {"output": 0, "value": 1}
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
-        L = C.CDLL(LIB)
-        L.emu_hist_batch_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
-                                          C.c_uint32, C.c_int, C.c_uint32, C.c_int64, C.c_void_p, C.c_uint64,
-                                          C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
-        L.emu_hist_batch_wire.restype = C.c_int
-        L.emu_hist_event_shares.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
-                                            C.c_void_p, C.c_int, C.c_void_p]
-        L.emu_hist_event_shares.restype = C.c_int
-        L.emu_hist_set_hot_slots.argtypes = [C.c_uint32]
-        _lib = L
-    return _lib
 
 
 def hist(wire, charwise, mode, key, text, offs, n_hist, hot_n=0, kernel=3, seg_len=0, hist_smem=1024, out=None):

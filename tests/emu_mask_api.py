@@ -1,27 +1,10 @@
-"""ctypes binding of tests/emu_mask/libdach_emu_mask.so: masked text (dach_dev_mask_batch) on the kernels' lane logic
-compiled for the CPU (test infrastructure only), and the reference the mask tests compare against."""
+"""Masked text (dach_dev_mask_batch) on the CPU emulation of the kernels' lane logic, tests/emu/libdach_emu.so
+(test infrastructure only), and the reference the mask tests compare against."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-EMU_DIR = os.path.join(_HERE, "emu_mask")
-LIB = os.path.join(EMU_DIR, "libdach_emu_mask.so")
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
-        L = C.CDLL(LIB)
-        L.emu_mask_batch_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64,
-                                          C.c_uint8, C.c_uint32, C.c_int, C.c_uint32, C.c_void_p, C.POINTER(C.c_int)]
-        L.emu_mask_batch_wire.restype = C.c_int
-        _lib = L
-    return _lib
+from emu_api import lib
 
 
 def mask(wire, charwise, mode, text, offs, fill, hot_n=0, kernel=3, seg_len=0, out=None):

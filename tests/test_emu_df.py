@@ -1,4 +1,4 @@
-"""Per-pattern document frequencies (dach_dev_df_batch) on the kernels' lane logic compiled for the CPU (tests/emu_df),
+"""Per-pattern document frequencies (dach_dev_df_batch) on the kernels' lane logic compiled for the CPU (tests/emu),
 against the oracle's per-haystack match lists: np.unique of the (haystack, key) pairs, then a bincount.  No GPU needed;
 tests/test_gpu_df.py runs the same checks on the device."""
 import json

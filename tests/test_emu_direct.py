@@ -1,12 +1,10 @@
-"""StdMachine3's direct matches path on the CPU emulation in tests/emu_direct: a lane stores each event into its block
+"""StdMachine3's direct matches path on the CPU emulation in tests/emu: a lane stores each event into its block
 at the landing that makes it, or keeps it pending for the service phase (no block with room, or a list length of 255
 or more); placement (k_expand) expands the blocks.  Checked against the oracle on the golden vectors, random batches,
 forced segments, stream chunks, ROOT's empty pattern, long lists, the pool / out_cap overflow protocol and items that
-end exactly on a block boundary; and against the queue path (tests/emu_events) for the number of blocks taken."""
-import ctypes as C
+end exactly on a block boundary; and against the queue path for the number of blocks taken."""
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -16,50 +14,14 @@ import oracle_api as O
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = json.load(open(os.path.join(HERE, "golden", "search_tests.json"), encoding="utf-8"))
-EMU_DIR = os.path.join(HERE, "emu_direct")
 MODE = {"find_iter": 0, "find_overlapping_iter": 1, "find_overlapping_no_suffix_iter": 2}
 ORC_MODE = {0: O.FIND, 1: O.FIND_OVERLAPPING, 2: O.FIND_OVERLAPPING_NO_SUFFIX}
 HOT = (0, 256, 1 << 16)
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
-        L = C.CDLL(os.path.join(EMU_DIR, "libdach_emu_direct.so"))
-        L.emu_direct_scan_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
-                                           C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
-                                           C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
-        L.emu_direct_scan_wire.restype = C.c_int
-        _lib = L
-    return _lib
 
 
 def scan(wire, mode, text, offs, hot_n=0, seg_len=0, seg_from=0, pool_blocks=None, out_cap=None, state=None, pos=None):
     """emu_events_api.scan's contract on the direct path: (rc, matches, out_offs, needed, blocks_used)."""
-    wire_a = np.frombuffer(wire, dtype=np.uint8)
-    text = np.ascontiguousarray(text, dtype=np.uint8)
-    offs = np.ascontiguousarray(offs, dtype=np.uint64)
-    n = len(offs) - 1
-    cap = int(out_cap) if out_cap is not None else 1 << 12
-    pad = text if text.size else np.zeros(16, dtype=np.uint8)
-    while True:
-        pb = int(pool_blocks) if pool_blocks is not None else cap // 30 + n + (text.size // seg_len + 1 if seg_len else 0) + 16
-        saved = state.copy() if state is not None else None
-        out = np.zeros(max(cap, 1), dtype=Q.MATCH_DTYPE)
-        oo = np.zeros(n + 1, dtype=np.uint64)
-        need, used = C.c_uint64(), C.c_uint32()
-        rc = lib().emu_direct_scan_wire(wire_a.ctypes.data, wire_a.size, mode, pad.ctypes.data, offs.ctypes.data, n, hot_n,
-                                        seg_len, seg_from, pb, state.ctypes.data if state is not None else None,
-                                        pos.ctypes.data if pos is not None else None, out.ctypes.data, cap, oo.ctypes.data,
-                                        C.byref(need), C.byref(used))
-        if rc == 6 and out_cap is None and pool_blocks is None:
-            if state is not None:
-                state[:] = saved
-            cap = max(cap * 2, int(need.value))
-            continue
-        return rc, out[: need.value] if rc == 0 else None, oo, int(need.value), int(used.value)
+    return Q.scan(wire, mode, text, offs, hot_n, seg_len, seg_from, pool_blocks, out_cap, state, pos, direct=True)
 
 
 def triples(m):

@@ -1,4 +1,4 @@
-"""StdMachine3's matches path with event blocks, on the CPU emulation in tests/emu_events: the drain stores
+"""StdMachine3's matches path with event blocks, on the CPU emulation in tests/emu: the drain stores
 (end, slot | list length) events, blocks are handed out per warp, placement (k_expand) expands them.  Checked
 against the oracle on the golden vectors, random batches, segments and stream chunks, and on what only this path
 has: output lists of 255 and more (the length byte's escape), warm-up events that must not be stored, and the pool /

@@ -1,4 +1,4 @@
-"""Per-pattern histograms (dach_dev_hist_batch) on the kernels' lane logic compiled for the CPU (tests/emu_hist), against
+"""Per-pattern histograms (dach_dev_hist_batch) on the kernels' lane logic compiled for the CPU (tests/emu), against
 the oracle's match lists.  No GPU needed; tests/test_gpu_hist.py runs the same checks on the device."""
 import json
 import os
@@ -152,12 +152,12 @@ def test_hist_smem_sizes_and_hot_regions(hot_slots):
     rng = np.random.default_rng(88 + hot_slots)
     pats = sorted(set(rand_patterns(rng, 1200, 5, 8)))
     text, offs = _batch(rng, 5, 16, 600)
-    H.lib().emu_hist_set_hot_slots(hot_slots)
+    H.lib().emu_set_hot_slots(hot_slots)
     try:
         for mode in (0, 1, 2):
             check(pats, False, 0, mode, text, offs, configs=[(256, 3, hs) for hs in (0, 1, 7, 256, 4096, 1 << 24)])
     finally:
-        H.lib().emu_hist_set_hot_slots(65536)
+        H.lib().emu_set_hot_slots(65536)
 
 
 def test_accumulates_across_batches():

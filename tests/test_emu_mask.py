@@ -1,4 +1,4 @@
-"""Masked text (dach_dev_mask_batch) on the kernels' lane logic compiled for the CPU (tests/emu_mask), against the
+"""Masked text (dach_dev_mask_batch) on the kernels' lane logic compiled for the CPU (tests/emu), against the
 oracle's match lists turned into spans.  No GPU needed; tests/test_gpu_mask.py runs the same checks on the device."""
 import json
 import os

@@ -1,41 +1,23 @@
 """The ordered event placement from block descriptors and two-entry output lists, on the CPU restatement in
-tests/emu_place: the pairs table against the chain walk of the outputs for every output record (C2 and C3 automata,
+tests/emu: the pairs table against the chain walk of the outputs for every output record (C2 and C3 automata,
 lists of three, 255 and more, ROOT's empty pattern), and the placement against the oracle -- golden vectors, random
 batches with forced segments, long lists, a pad of 0 to 3 words before the output, 1 to 8 blocks per warp, and the
 pool / out_cap overflow protocol."""
-import ctypes as C
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import emu_events_api as Q
+from emu_api import lib
 import oracle_api as O
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = json.load(open(os.path.join(HERE, "golden", "search_tests.json"), encoding="utf-8"))
-EMU_DIR = os.path.join(HERE, "emu_place")
 MODE = {"find_iter": 0, "find_overlapping_iter": 1, "find_overlapping_no_suffix_iter": 2}
 ORC_MODE = {0: O.FIND, 1: O.FIND_OVERLAPPING, 2: O.FIND_OVERLAPPING_NO_SUFFIX}
 CLASS_SHIFT = 30
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
-        L = C.CDLL(os.path.join(EMU_DIR, "libdach_emu_place.so"))
-        L.emu_place_scan_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
-                                          C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
-                                          C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
-        L.emu_place_scan_wire.restype = C.c_int
-        L.emu_place_tables.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint64]
-        L.emu_place_tables.restype = C.c_int64
-        _lib = L
-    return _lib
 
 
 def tables(wire):
@@ -69,24 +51,7 @@ def check_pairs(wire):
 
 def scan(wire, mode, text, offs, u=4, pad=0, seg_len=0, seg_from=0, pool_blocks=None, out_cap=None):
     """(rc, matches, out_offs, needed, blocks_used), growing out_cap and the pool until the batch fits unless given"""
-    wire_a = np.frombuffer(wire, dtype=np.uint8)
-    text = np.ascontiguousarray(text, dtype=np.uint8)
-    offs = np.ascontiguousarray(offs, dtype=np.uint64)
-    n = len(offs) - 1
-    cap = int(out_cap) if out_cap is not None else 1 << 12
-    pad_t = text if text.size else np.zeros(16, dtype=np.uint8)
-    while True:
-        pb = int(pool_blocks) if pool_blocks is not None else cap // 30 + n + (text.size // seg_len + 1 if seg_len else 0) + 16
-        out = np.zeros(max(cap, 1), dtype=Q.MATCH_DTYPE)
-        oo = np.zeros(n + 1, dtype=np.uint64)
-        need, used = C.c_uint64(), C.c_uint32()
-        rc = lib().emu_place_scan_wire(wire_a.ctypes.data, wire_a.size, mode, pad_t.ctypes.data, offs.ctypes.data, n, 0,
-                                       seg_len, seg_from, pb, None, None, out.ctypes.data, cap, u, pad, oo.ctypes.data,
-                                       C.byref(need), C.byref(used))
-        if rc == 6 and out_cap is None and pool_blocks is None:
-            cap = max(cap * 2, int(need.value))
-            continue
-        return rc, out[: need.value] if rc == 0 else None, oo, int(need.value), int(used.value)
+    return Q.scan(wire, mode, text, offs, 0, seg_len, seg_from, pool_blocks, out_cap, direct=True, place_u=u, place_pad=pad)
 
 
 def batch(hays):

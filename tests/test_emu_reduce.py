@@ -1,5 +1,5 @@
 """Counts and first matches (dach_dev_count_batch / dach_dev_first_batch) on the kernels' lane logic compiled for the
-CPU (tests/emu_reduce), against the oracle.  No GPU needed; tests/test_gpu_reduce.py runs the same checks on the device."""
+CPU (tests/emu), against the oracle.  No GPU needed; tests/test_gpu_reduce.py runs the same checks on the device."""
 import json
 import os
 

@@ -1,43 +1,23 @@
 """Counts, first matches and per-pattern histograms of stream chunks (dach_dev_count_stream / dach_dev_first_stream /
-dach_dev_hist_stream) on the kernels' lane logic compiled for the CPU (tests/emu_stream_rk), against the
+dach_dev_hist_stream) on the kernels' lane logic compiled for the CPU (tests/emu), against the
 crate's steppers (oracle) driven over each whole stream.  No GPU needed; tests/test_gpu_stream_rk.py runs the device
 forms against dach_dev_scan_stream."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import emu_api as EM
 import emu_reduce_api as E
+from emu_api import lib
 import oracle_api as O
 from cases import MIXED
 
 FIND, OVERLAPPING = 0, 1
 COUNT, FIRST, HIST = 1, 2, 3
-HERE = os.path.dirname(os.path.abspath(__file__))
 STEPPER = {FIND: O.FIND_STEPPER, OVERLAPPING: O.FIND_OVERLAPPING_STEPPER}
 NONE = (0xFFFFFFFF, 0xFFFFFFFF, 0xFFFFFFFF)
 KEY = {"output": 0, "value": 1}  # dach_hist_key
-
-
-_LIB = None
-
-
-def lib():
-    """tests/emu_stream_rk/libdach_emu_stream_rk.so, built on first use."""
-    global _LIB
-    if _LIB is None:
-        subprocess.check_call(["make", "-C", os.path.join(HERE, "emu_stream_rk"), "-s"])
-        L = C.CDLL(os.path.join(HERE, "emu_stream_rk", "libdach_emu_stream_rk.so"))
-        L.emu_rk_stream_wire.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                         C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int, C.c_int64, C.c_void_p,
-                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
-        L.emu_rk_stream_wire.restype = C.c_int
-        L.emu_stream_rk_set_hot_slots.argtypes = [C.c_uint32]
-        _LIB = L
-    return _LIB
 
 
 def _call(wire, cw, mode, rk, text, offs, state, pos=None, key=0, hot_n=0, kernel=3, hist_smem=1024, counts=None, first=None,
@@ -211,12 +191,10 @@ def test_bytewise_streams_without_a_hot_region(mode):
     pats, streams, cuts = bytewise_streams(1)
     opma = O.OraclePma.build(pats)
     wire = opma.serialize()
-    lib().emu_stream_rk_set_hot_slots(0)
     EM.lib().emu_set_hot_slots(0)
     try:
         state = run_case(wire, False, mode, streams, cuts, opma, _hist_sizes(wire, False), seed=21 + mode)
     finally:
-        lib().emu_stream_rk_set_hot_slots(65536)
         EM.lib().emu_set_hot_slots(65536)
     for i, s in enumerate(streams):
         assert int(state[i]) == opma.state_after(s, find_mode=(mode == FIND)), i

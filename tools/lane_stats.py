@@ -7,7 +7,7 @@ No GPU needed.  Usage: python tools/lane_stats.py [C2|C3|C5 ...]
 
 reports instead how the lane machines' output events (what a HIST scan counts per state) spread over the compact
 slots: the share on the 1 / 64 / 1024 / 4096 busiest slots and on the leading 1024 / 4096 slots (what option hist_smem
-counts in shared memory), from tests/emu_hist.
+counts in shared memory), from the same emulation's HIST scan.
 
     python tools/lane_stats.py --lists [C3 C2 ...]
 
@@ -20,8 +20,8 @@ head record's chain word instead), from the oracle's matches.
 
 reports what a document-frequency window holds (dach_dev_df_batch, DESIGN.md section 4.9): the distinct (haystack,
 state) pairs the lane machine puts into the first set and the distinct (haystack, key) pairs of the second, per MiB of
-text, on 4 MiB of the workload's own haystacks, from tests/emu_df -- and so how much text one window of option
-df_pairs pairs covers."""
+text, on 4 MiB of the workload's own haystacks, from the same emulation's DF scan -- and so how much text one window
+of option df_pairs pairs covers."""
 import ctypes as C
 import os
 import sys
